@@ -1,11 +1,11 @@
 #!/usr/bin/env python3
-"""bench.py — RGB-D frames/s of the PlanarSLAM per-frame hot path on B200 (BASELINE.json metric).
+"""bench.py — RGB-D frames/s of the PlanarSLAM per-frame hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
-A "step" = one pass of the hot path over 7104 frames of a 256-frame synthetic 640x480 RGB-D sequence ("room corner", planarslam_b200/synth.py): four library
-calls of 1776 frames for ORB / PEAC / PoseOptimization and two of 3552 for LSD, so that every call of a one-warp-per-frame kernel is exactly one resident wave.
+A "step" = one pass of the hot path over 6336 frames of a 256-frame synthetic 640x480 RGB-D sequence ("room corner", planarslam_b200/synth.py): four library
+calls of 1584 frames for ORB / PEAC / PoseOptimization and two of 3168 for LSD, so that every call of a one-warp-per-frame kernel is exactly one resident wave.
 With PSLAM_EXTRAS=1 (default) the extractors are followed by what the Frame constructor and Tracking run on their output: ComputeStereoFromRGBD, MatchORBPoints
 against the previous frame, the key-frame exchange, LBD descriptors, isLineGood, the ComputePlanes post-processing, surface normals, TrackManhattanFrame.
 Frames are independent units, so ranks shard them with no data-path collective (weak scaling: every rank processes FRAMES_PER_STEP frames per step); the
@@ -45,14 +45,16 @@ AREA = (W * H) // (640 * 480)                                   # frames of conf
 K_CAM = tuple(k * W / 640.0 for k in (535.4, 539.2, 320.1, 247.6))
 # Frames per library call (context max_batch).  The serial-order kernels run one warp per frame, so throughput scales with
 # frames in flight; the default is one full wave of the clustering kernel (pslam_peac_wave_frames: SMs x resident CTAs/SM,
-# 1776 on a 148-SM B200), set in main().  1776 frames = 1.6 GB of gray+depth input >> 126 MB L2.
+# 1584 on a 132-SM H100), set in main().  1584 frames = 1.5 GB of gray+depth input >> 50 MB L2.
 SUB_BATCH = int(os.environ.get("PSLAM_SUB_BATCH", "0"))
-DEFAULT_WAVE = 1776 // min(AREA, 2)                                    # 148 SMs x 12 resident clustering CTAs (a quarter of a wave at 1280x960: device memory per frame is 4x)
+DEFAULT_WAVE = 1584 // AREA                                            # 132 SMs x 12 resident clustering CTAs (a quarter of a wave at 1280x960: device memory per frame is 4x)
+E2E_WAVE = 1056 // AREA                                                # frames per context of the end-to-end leg: a full-family context holds ~31 MB per
+                                                                       # 640x480 frame, so two contexts of 1056 frames take ~65 GB of the 80 GB
 SUBS_PER_STEP = int(os.environ.get("PSLAM_SUBS", "4"))         # ORB / PEAC / pose library calls per step (LSD takes the whole step in one call:
                                                                # its one-warp-per-frame kernel needs 32 frames per SM in flight, PEAC clustering fits 12)
 FRAMES_PER_STEP = SUB_BATCH * SUBS_PER_STEP
-LSD_SUBS = int(os.environ.get("PSLAM_LSD_SUBS", "2" if AREA == 1 else "4"))          # LSD calls per step: 4 x 1776 = 2 x 3552 frames, i.e. every LSD call is exactly one wave of its
-                                                               # one-warp-per-frame kernel (24 resident CTAs per SM x 148), every PEAC call one wave of the clustering kernel (12 x 148)
+LSD_SUBS = int(os.environ.get("PSLAM_LSD_SUBS", "2" if AREA == 1 else "4"))          # LSD calls per step: 4 x 1584 = 2 x 3168 frames, i.e. every LSD call is exactly one wave of its
+                                                               # one-warp-per-frame kernel (24 resident CTAs per SM x 132), every PEAC call one wave of the clustering kernel (12 x 132)
 DISTINCT_FRAMES = int(os.environ.get("PSLAM_DISTINCT_FRAMES", "256"))   # distinct frames of the replayed sequence (rendered on the host cores by a process pool)
                                                                          # and distinct pose problems; the step's frames cycle through them
 
@@ -106,7 +108,7 @@ def _peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "datasheet"                 # H100 SXM HBM3
 
 
 def make_frames(n_distinct=DISTINCT_FRAMES, world=1):
@@ -426,6 +428,40 @@ def run_reference(args, rank, world):
     print(json.dumps(line))
 
 
+DUMP_FRAMES = 8             # frames per output that --dump-outputs writes: a fixed seeded sample (one step's outputs are several GB)
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(path, outs, counts):
+    """--dump-outputs: {name: (device tensor [frames, ...], valid entries per frame or None, record dtype or None)} -> path/<name>.npy in float32
+    (float64 for double and record outputs) for DUMP_FRAMES frames drawn with a fixed seed; entries past a frame's count are zeroed, since the buffers
+    are not cleared between calls.  counts: per-frame counts of the whole step, written in full.  Every value written is finite."""
+    from numpy.lib import recfunctions as rf
+    arrays = {}
+    for name, (t, cnt, dtype) in outs.items():
+        rows = np.sort(np.random.default_rng(0).choice(t.shape[0], min(DUMP_FRAMES, t.shape[0]), replace=False))
+        a = t.cpu().numpy()[rows]
+        if dtype is not None:
+            a = rf.structured_to_unstructured(np.ascontiguousarray(a).view(dtype).reshape(a.shape[:-1]), dtype=np.float64)
+        else:
+            a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        if cnt is not None:
+            c = cnt.cpu().numpy()
+            c = np.where(rows < len(c), c[np.minimum(rows, len(c) - 1)], 0)
+            a[np.arange(a.shape[1])[None, :] >= c[:, None]] = 0
+        arrays[name] = a
+    arrays.update({k: v.cpu().numpy().astype(np.float32) for k, v in counts.items()})
+    bad = [name for name, a in arrays.items() if not np.isfinite(a).all()]
+    if bad:
+        raise RuntimeError(f"--dump-outputs: non-finite values in {bad}")
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT:
+        raise RuntimeError(f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT} byte limit")
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def workload_config():
     return {"workload": f"{W}x{H} synthetic RGB-D sequence: ORB ({NFEATURES} feats, 8 levels) + LSD line segments (REFINE_ADV, 40 longest -> KeyLines + "
                         "line functions) + PEAC planes + PoseOptimization (1000 point + 40 line (80 edges) + 6 plane "
@@ -442,8 +478,11 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write what the timed path computed in its last step to DIR/<name>.npy")
     ap.add_argument("--cpu-worker", default=None, help=argparse.SUPPRESS)       # internal: child process of the CPU arm
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.cpu_worker:
         cpu_worker_main(json.loads(args.cpu_worker))
         return
@@ -469,7 +508,7 @@ def main():
     global SUB_BATCH, FRAMES_PER_STEP
     if SUB_BATCH <= 0:
         probe = Context(W, H, 1, device=local_rank)
-        SUB_BATCH = (int(probe.L.pslam_peac_wave_frames(probe.h)) or 1776) // min(AREA, 2)          # config 5: half a wave per call (device memory per frame is 4x)
+        SUB_BATCH = (int(probe.L.pslam_peac_wave_frames(probe.h)) or 1584) // AREA          # config 5: a quarter of a wave per call (device memory per frame is 4x)
         del probe
     FRAMES_PER_STEP = SUB_BATCH * SUBS_PER_STEP
     assert LSD_SUBS <= SUBS_PER_STEP
@@ -740,6 +779,34 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms_max = float(t.item())
     value = world * FRAMES_PER_STEP * args.steps / (ms_max / 1e3)
+    if args.dump_outputs and rank == 0:        # before the roofline pass below, which reruns the first sub-batch into the same buffers
+        o_last = (SUBS_PER_STEP - 1) * SUB_BATCH
+        outs = {}
+        if "orb" in STAGES:
+            outs.update(orb_keypoints=(d_kps, d_n[o_last:], KEYPOINT_DTYPE), orb_descriptors=(d_desc, d_n[o_last:], None))
+            if EXTRAS:
+                outs.update(stereo_u_right=(d_ur, d_n[o_last:], None), stereo_depth=(d_dz, d_n[o_last:], None),
+                            match_prev_index=(d_midx, d_n[o_last + 1:], None), match_prev_distance=(d_mdist, d_n[o_last + 1:], None))
+        if "peac" in STAGES:
+            outs.update(peac_labels=(d_labels, None, None), peac_planes=(d_planes, d_npl[o_last:], PLANE_DTYPE),
+                        peac_members=(d_members, d_moff.gather(1, d_npl[o_last:o_last + SUB_BATCH, None].long())[:, 0], None))
+            if EXTRAS:
+                outs.update(planes_src=(d_pp_src, d_pp_n, None), planes_coef=(d_pp_coef, d_pp_n, None),
+                            planes_points=(d_pp_pts, d_pp_off.gather(1, d_pp_n[:, None].long())[:, 0], None),
+                            manhattan=(d_mres, None, MANHATTAN_RESULT_DTYPE),
+                            # a normal PCL leaves undefined is NaN: written as 0, with the mask of defined normals beside it
+                            surface_normals=(torch.where(d_sn8.isfinite(), d_sn8, 0.0), None, None),
+                            surface_normals_defined=(d_sn8[..., :3].isfinite().all(-1).float(), None, None))
+        if "lsd" in STAGES:
+            outs.update(keylines=(d_kl, d_nkl, KEYLINE_DTYPE), line_functions=(d_lf, d_nkl, None))
+            if EXTRAS:
+                outs.update(line_descriptors=(d_ldesc, d_nkl, None), lines3d=(d_l3d, d_nkl, LINE3D_DTYPE))
+        if "pose" in STAGES:
+            r = opt.fetch()
+            outs.update(pose_Tcw=(torch.from_numpy(np.stack([q["Tcw_d"] for q in r])), None, None),
+                        pose_inliers=(torch.tensor([q["n_inliers"] for q in r]), None, None))
+        counts = {"orb_n": d_n, "peac_n_planes": d_npl, "lsd_n_keylines": d_nkl}
+        dump_outputs(args.dump_outputs, outs, {k: v for k, v in counts.items() if k.split("_")[0] in STAGES})
 
     # ---- per-kernel roofline pass (event-bracketed launches, same workload, outside the timed regions) ----
     # one stage family at a time, so a launch's duration is not inflated by kernels of the other two streams
@@ -767,16 +834,9 @@ def main():
     for v in per_kernel.values():
         v["share"] = round(v["ms_total"] / tot, 4)
     dom = max(per_kernel, key=lambda k: per_kernel[k]["ms_total"])
-    # DRAM bytes per frame of the dominant kernels from the committed round-2 `ncu --set full` captures (dram__bytes_read.sum + dram__bytes_write.sum of one
-    # launch / its frames: profiles/r2_ncu_full_lsd_kernels.csv at 3552 frames, profiles/r2_ncu_full_peac_kernels.csv at 1776; k_peac_flood from
-    # profiles/r1_ncu_full_summary.csv at 296 - its round-2 capture returned no DRAM counters), scaled to this run's frames per launch
-    # (k_lsd_regions re-captured after its last change at the benchmark launch size: 99.141 + 9.583 GB per 3552 frames, profiles/r2_final_ncu_full_lsd_regions_peac_flood.csv)
-    NCU_DRAM_BYTES_PER_FRAME = {"lsd_regions": (99.140878e9 + 9.582504e9) / 3552, "peac_cluster": (8.573231e9 + 3.334866e9) / 1776,
-                                "peac_flood": (4.953115e9 + 1.131992e9) / 296, "lsd_improve": (3.480971e9 + 1.401838e9) / 3552}
-    traffic = NCU_DRAM_BYTES_PER_FRAME.get(dom)
     roofline = {"kernel": dom, "bound": "hbm", "achieved": per_kernel[dom]["achieved_gbs"], "peak": peak, "unit": "GB/s",
                 "frac": round(per_kernel[dom]["achieved_gbs"] / peak, 6),
-                "traffic": int(traffic * FRAMES_PER_STEP / per_kernel[dom]["launches"]) if traffic else None, "peak_kind": peak_kind,
+                "traffic": None, "peak_kind": peak_kind,
                 "note": "serial-order kernels (quadtree, AHC, PEAC / LSD region growing, LM) run one warp/CTA per frame: latency-bound, see DESIGN.md",
                 "per_kernel": per_kernel}
 
@@ -832,7 +892,7 @@ def main():
     if frame_e2e:
         # The call a replay driver makes per batch is the Frame constructor's compute, pslam_frame_construct_batch: host frames in (uploaded once), every Frame
         # product out.  Two contexts on two host threads take alternate sub-batches, so one batch's copies overlap the other's kernels; PoseOptimization runs on
-        # a third thread as before.  The device-resident leg's contexts and buffers are released first (two full-family contexts take ~110 GB).
+        # a third thread as before.  The device-resident leg's contexts and buffers are released first (two full-family contexts take ~65 GB).
         barrier()
         xch = None
         del d_gray, d_depth, d_kps, d_desc, d_labels, d_planes, d_members, d_moff, d_kl, d_lf, d_ur, d_dz, d_midx, d_mdist, d_good, d_ldesc, d_l3d, d_pp_coef, d_pp_pts
@@ -841,11 +901,9 @@ def main():
             c.close()
         torch.cuda.empty_cache()
         from planarslam_b200.frame import ConstructFrames, FrameOutputs
-        # PSLAM_E2E_CONTEXTS contexts (default 2) of 2 * SUB_BATCH / contexts frames each - the device memory of two full sub-batches either way.  Measured on B200
-        # (profiles/r2_exp_e2e_*contexts.json): two contexts of 1776 frames 5.2 k frames/s, four of 888 frames 4.6 k - smaller calls leave the one-warp-per-frame
-        # kernels with quarter-wave launches.
+        # PSLAM_E2E_CONTEXTS contexts (default 2) of 2 * E2E_WAVE / contexts frames each - the device memory of two E2E_WAVE batches either way.
         E2E_CTX = max(2, int(os.environ.get("PSLAM_E2E_CONTEXTS", "2")))
-        E2E_BATCH = max(1, 2 * min(SUB_BATCH, int(os.environ.get("PSLAM_E2E_WAVE", str(DEFAULT_WAVE)))) // E2E_CTX)      # (two contexts of one clustering wave each: ~110 GB)
+        E2E_BATCH = max(1, 2 * min(SUB_BATCH, int(os.environ.get("PSLAM_E2E_WAVE", str(E2E_WAVE)))) // E2E_CTX)
         E2E_CALLS = (FRAMES_PER_STEP + E2E_BATCH - 1) // E2E_BATCH
         fctx = [Context(W, H, E2E_BATCH, device=local_rank, nfeatures=NFEATURES) for _ in range(E2E_CTX)]
         fout = [FrameOutputs(c, E2E_BATCH, MAX_LINES, PP_CAP, normals=True, pinned=True) for c in fctx]

@@ -1,4 +1,4 @@
-/* pslam_abi.h — C ABI of the B200-native PlanarSLAM per-frame hot path (libpslam_b200.so).
+/* pslam_abi.h — C ABI of the H100-native PlanarSLAM per-frame hot path (libpslam_b200.so).
  *
  * The reference (yanyan-li/PlanarSLAM) has no plugin/FFI layer: its seam is a set of C++ methods called
  * from Frame / Tracking (SURVEY.md §8b).  Each entry point below replaces one of those methods with plain
@@ -8,7 +8,7 @@
  * never allocates caller-visible memory (the caller passes capacities); a context is bound to one GPU and is
  * used by one thread at a time (the reference calls ORB / LSD / PEAC from three threads: use one context
  * per thread, they are re-entrant across contexts).  There is NO CPU fallback: creation fails with
- * PSLAM_E_NO_DEVICE when no sm_100 device is present.
+ * PSLAM_E_NO_DEVICE when no sm_90 device is present.
  *
  * "_dev" variants take device pointers and enqueue on the context's stream without synchronising
  * (inputs already resident in HBM); the plain variants take host pointers, copy in, run, copy out and
@@ -26,7 +26,7 @@ extern "C" {
 typedef enum pslam_status {
     PSLAM_OK = 0,
     PSLAM_E_INVALID = -1,    /* bad argument (null pointer, size mismatch, unsupported parameter) */
-    PSLAM_E_NO_DEVICE = -2,  /* no CUDA device / not sm_100 */
+    PSLAM_E_NO_DEVICE = -2,  /* no CUDA device / not sm_90 */
     PSLAM_E_CUDA = -3,       /* CUDA runtime error; see pslam_last_error() */
     PSLAM_E_CAPACITY = -4,   /* an internal or caller capacity was exceeded (results truncated) */
     PSLAM_E_NCCL = -5

@@ -1,5 +1,5 @@
 // pslam_adapter.hpp — header-only C++ adapter that re-creates the reference's class interfaces on top of the C ABI
-// (include/pslam_abi.h), so Frame / Tracking can switch to the B200 path without changing their call sites.
+// (include/pslam_abi.h), so Frame / Tracking can switch to the GPU path without changing their call sites.
 //
 // This header carries the reference's method names and argument order over plain pointers / std::vector (no OpenCV, Eigen or PCL needed;
 // tests/test_adapter_compiles.py builds it).  The calls WITH the reference's own argument types (Frame*, KeyFrame*, cv::InputArray,
@@ -34,7 +34,7 @@ public:
         pslam_config cfg;
         if (overrides) cfg = *overrides; else pslam_default_config(&cfg, width, height, 1);
         cfg.width = width; cfg.height = height;
-        if (pslam_create(&cfg, &ctx_) != PSLAM_OK) throw std::runtime_error("pslam_create failed: no sm_100 GPU or bad configuration");
+        if (pslam_create(&cfg, &ctx_) != PSLAM_OK) throw std::runtime_error("pslam_create failed: no sm_90 GPU or bad configuration");
         cfg_ = cfg;
     }
     ~Context() { pslam_destroy(ctx_); }

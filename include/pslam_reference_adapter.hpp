@@ -68,7 +68,7 @@ inline pslam_ctx* context(int width = 640, int height = 480) {
         if (H.c) pslam_destroy(H.c);
         pslam_config cfg;
         pslam_default_config(&cfg, width, height, 1);
-        if (pslam_create(&cfg, &H.c) != PSLAM_OK) { H.c = nullptr; throw std::runtime_error("pslam_create failed: no sm_100 GPU"); }
+        if (pslam_create(&cfg, &H.c) != PSLAM_OK) { H.c = nullptr; throw std::runtime_error("pslam_create failed: no sm_90 GPU"); }
         H.w = width; H.h = height;
     }
     return H.c;
@@ -696,7 +696,7 @@ public:
             pslam_config cfg;
             pslam_default_config(&cfg, image.cols, image.rows, 1);
             cfg.nfeatures = nfeatures; cfg.scale_factor = scaleFactor; cfg.nlevels = nlevels; cfg.ini_th_fast = iniThFAST; cfg.min_th_fast = minThFAST;
-            if (pslam_create(&cfg, &ctx) != PSLAM_OK) { ctx = nullptr; throw std::runtime_error("pslam_create failed: no sm_100 GPU"); }
+            if (pslam_create(&cfg, &ctx) != PSLAM_OK) { ctx = nullptr; throw std::runtime_error("pslam_create failed: no sm_90 GPU"); }
             w = image.cols; h = image.rows;
         }
         const int cap = pslam_orb_max_keypoints(ctx);

@@ -1,6 +1,6 @@
 """ctypes binding of libpslam_b200.so (the C ABI in include/pslam_abi.h).
 
-There is deliberately no fallback: if the CUDA library is missing or no sm_100 GPU is present the
+There is deliberately no fallback: if the CUDA library is missing or no sm_90 GPU is present the
 import / context creation fails loudly.
 """
 from __future__ import annotations
@@ -155,7 +155,7 @@ class Context:
         h = C.c_void_p()
         rc = L.pslam_create(C.byref(cfg), C.byref(h))
         if rc != PSLAM_OK:
-            raise PslamError(rc, "pslam_create failed (no sm_100 GPU, or invalid configuration; see stderr)")
+            raise PslamError(rc, "pslam_create failed (no sm_90 GPU, or invalid configuration; see stderr)")
         self.h = h
         self.L = L
 

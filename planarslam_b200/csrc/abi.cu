@@ -50,7 +50,7 @@ int pslam_create(const pslam_config* cfg, pslam_ctx** out) {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || cfg->device < 0 || cfg->device >= ndev) return PSLAM_E_NO_DEVICE;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 10) return PSLAM_E_NO_DEVICE;  // sm_100a only
+    if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 9) return PSLAM_E_NO_DEVICE;   // sm_90a only
     pslam_ctx* c = new (std::nothrow) pslam_ctx();
     if (!c) return PSLAM_E_INVALID;
     c->cfg = *cfg;

@@ -1,4 +1,4 @@
-// DBoW2 vocabulary transform on sm_100a: TemplatedVocabulary<FORB::TDescriptor, FORB>::transform(features, BowVector&, FeatureVector&,
+// DBoW2 vocabulary transform on sm_90a: TemplatedVocabulary<FORB::TDescriptor, FORB>::transform(features, BowVector&, FeatureVector&,
 // levelsup) (Thirdparty/DBoW2/DBoW2/TemplatedVocabulary.h:1125-1193, per-feature descent :1213-1252) as Frame::ComputeBoW /
 // KeyFrame::ComputeBoW use it (TF_IDF weights, L1 normalisation, levelsup = 4).
 //   k_bow_descend   one warp per feature: at every level the lanes take one child each (k <= 32), 256-bit Hamming distance, warp

@@ -1,4 +1,4 @@
-// Local bundle adjustment on sm_100a: one CTA per problem runs the reference's whole LocalBundleAdjustment numeric core
+// Local bundle adjustment on sm_90a: one CTA per problem runs the reference's whole LocalBundleAdjustment numeric core
 // (src/Optimizer.cc:2361-2460 around g2o's BlockSolver_6_3 + Levenberg): optimize(5) with Huber kernels, chi-square gating,
 // optimize(10) without kernels.  Every stage is a block-wide loop over a static work list built at pack time, so all sums
 // have a fixed order (deterministic, and - up to libm ulps in sin/cos/atan2 - the order the CPU restatement uses):

@@ -63,7 +63,7 @@ static void lba_plane_from_float4(const float* v, double out[4]) {     // Conver
     for (int i = 0; i < 4; ++i) out[i] = p[i];
 }
 
-static const int LBA_SMEM_BUDGET = 200 * 1024;      // dynamic shared memory we are willing to ask for (227 KB per CTA on sm_100)
+static const int LBA_SMEM_BUDGET = 200 * 1024;      // dynamic shared memory we are willing to ask for (227 KB per CTA on sm_90)
 
 int lba_pack_upload(pslam_ctx* c, const pslam_lba_problem* probs, int nprob) {
     if (!c->lba) c->lba = new LbaBuffers();

@@ -1,4 +1,4 @@
-// Brute-force Hamming matching of 256-bit descriptors (ORB rBRIEF, LBD) for sm_100a, batched over frames.
+// Brute-force Hamming matching of 256-bit descriptors (ORB rBRIEF, LBD) for sm_90a, batched over frames.
 //
 // Reference semantics: ORBmatcher::DescriptorDistance src/ORBmatcher.cc:1712-1728; ORBmatcher::MatchORBPoints :1332-1394
 // (cv::BFMatcher(NORM_HAMMING).match, then keep dist < max(2*min_dist, 15)); LSDmatcher::SearchByDescriptor

@@ -1,4 +1,4 @@
-// ORB extraction kernels for sm_100a (batched over frames: blockIdx.y or .z selects the frame).
+// ORB extraction kernels for sm_90a (batched over frames: blockIdx.y or .z selects the frame).
 //
 // Reference semantics (file:line under /root/reference): ComputePyramid src/ORBextractor.cc:1107-1132,
 // ComputeKeyPointsOctTree :765-853, DistributeOctTree :539-763, IC_Angle :77-104, GaussianBlur call :1086,
@@ -74,7 +74,7 @@ __device__ __forceinline__ int fast_score(const uint8_t (*win)[FAST_WIN_MAX + 4]
         if (nb < 2 && nd < 2) return 0;
     }
     // d = centre - circle (dark arcs), e = circle - centre (bright arcs).  Both polarities use min-chains only:
-    // nvcc 12.9 / sm_100a miscompiles max(x, -y) when it is folded into a 3-input VIMNMX (observed on B200:
+    // nvcc 12.9 has been seen to miscompile max(x, -y) when it is folded into a 3-input VIMNMX (observed on sm_100a:
     // max(0, max(-4, -203)) evaluated to 203), so no negation may appear inside a min/max operand here.
     int d[16], e[16];
     const int c1 = win[y + 3][x + 1], c2 = win[y + 2][x + 2], c3 = win[y + 1][x + 3], c5 = win[y - 1][x + 3];

@@ -1,4 +1,4 @@
-// PEAC plane extraction kernels for sm_100a (batched over frames).
+// PEAC plane extraction kernels for sm_90a (batched over frames).
 //
 // Reference semantics (file:line under /root/reference): PlaneDetection::readDepthImage src/PlaneExtractor.cpp:26-57,
 // ImagePointCloud::get include/PlaneExtractor.h:25-33, ahc::PlaneSeg ctor include/peac/AHCPlaneSeg.hpp:211-285,

@@ -1,4 +1,4 @@
-// Pose optimisation on sm_100a: one CTA per frame runs the reference's whole PoseOptimization — four rounds of
+// Pose optimisation on sm_90a: one CTA per frame runs the reference's whole PoseOptimization — four rounds of
 // Levenberg-Marquardt (<= 10 iterations each, g2o's control flow) over point / line / plane unary edges with chi-square
 // re-classification between rounds.  Edges are evaluated edge-parallel (one thread per edge, strided), the 6x6 normal
 // equations (21 unique entries of J^T W J plus 6 of J^T W r) and the robust chi2 are reduced with warp shuffles and a

@@ -50,8 +50,8 @@ struct OrbGeom {
 // TMA-staged Gaussian blur of the ORB path (orb_kernels.cuh k_blur_tma): tile / box geometry and the kernel parameter block
 #define BT_W 128
 #define BT_H 64
-#define BT_BOX_W 160          // 16 + 128 + 3 rounded up to 16: the box must START at a 16-byte multiple of the row (measured on B200: a start column that is not a
-                              // multiple of 16 bytes raises "illegal instruction", tools/dbg/tma_min.cu), so it starts 16 columns left of the tile
+#define BT_BOX_W 160          // 16 + 128 + 3 rounded up to 16: the box must START at a 16-byte multiple of the row (a start column that is not a
+                              // multiple of 16 bytes raised "illegal instruction" in tools/dbg/tma_min.cu), so it starts 16 columns left of the tile
 #define BT_X_PAD 16
 #define BT_BOX_H 70
 struct BlurTmaParams {

@@ -1,4 +1,4 @@
-// Projection-guided descriptor search for sm_100a (one frame + one map snapshot per call; frames of a replayed
+// Projection-guided descriptor search for sm_90a (one frame + one map snapshot per call; frames of a replayed
 // sequence are issued back to back on the context's stream).
 //
 // Reference semantics: Frame::AssignFeaturesToGrid / PosInGrid src/Frame.cc:155-168,526-535; Frame::GetFeaturesInArea :440-489;

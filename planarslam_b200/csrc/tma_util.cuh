@@ -1,4 +1,4 @@
-// TMA (cp.async.bulk.tensor) + mbarrier helpers for sm_100a, and the host-side tensor-map encoder.
+// TMA (cp.async.bulk.tensor) + mbarrier helpers for sm_90a, and the host-side tensor-map encoder.
 //
 // Image / depth tiles are staged into shared memory by the tensor memory accelerator: one elected thread arms an mbarrier with the
 // byte count of the box and issues the bulk tensor copy; the copy engine zero-fills whatever part of the box lies outside the tensor

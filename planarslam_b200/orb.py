@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's ORBextractor (include/ORBextractor.h:47-116) on top of the C ABI.
 
 Same constructor arguments, getters and call shape as the reference class; the work happens in
-libpslam_b200.so (CUDA, sm_100a).  Images are numpy uint8 arrays, keypoints come back as a structured
+libpslam_b200.so (CUDA, sm_90a).  Images are numpy uint8 arrays, keypoints come back as a structured
 array layout-compatible with cv::KeyPoint (28 bytes), descriptors as an N x 32 uint8 array.
 """
 from __future__ import annotations

@@ -3,8 +3,8 @@
 Bar (BASELINE.json north_star): SE3 pose within 1e-4 rad / 1e-3 m of the reference path after the same LM iteration
 count.  The two implementations share the summation order of H_ll, H_pp, b and of the Schur terms; they differ in libm
 ulps (sin / cos / atan2 inside the plane edges' numeric Jacobians, se3 exp) and in the tree-shaped chi2 reductions, so the
-tolerances used here are far tighter than the bar: 1e-6 rad / 1e-6 m on key-frame poses (measured on B200: 3e-8 rad / 8e-8 m),
-1e-4 m on landmarks (median 1.5e-7 m; two-view points at 4 m depth amplify the pose difference to ~1e-5 m), identical erase
+tolerances used here are far tighter than the bar: 1e-6 rad / 1e-6 m on key-frame poses,
+1e-4 m on landmarks (two-view points at 4 m depth amplify the pose difference to ~1e-5 m), identical erase
 lists and identical LM iteration / trial counts.  A points-only problem (no libm on the path beyond se3 exp's small-angle
 branch) must agree bit for bit."""
 import numpy as np

@@ -2,8 +2,7 @@
 enumeration (pslam_lsd_set_rect_enumeration(ctx, 1)) - compiled for the HOST with g++ and compared with the oracle's statement
 of the same enumeration (oracle/lsd.cc rect_rows_cv4, itself pinned against cv2 4.13 by tests/test_oracle_lsd.py).  The header
 is plain double arithmetic (nvcc builds it with --fmad=false), so host spans = device spans; the device-side pixel loop is the
-same as the validated one of the published iterator.  This is the only check that variant has had so far: no GPU time was left
-to run it on a B200 in round 1 (DESIGN.md section 5.7)."""
+same as the validated one of the published iterator; tests/test_lsd_gpu.py runs the device side against the oracle."""
 import ctypes as C
 import os
 import subprocess

@@ -1,7 +1,7 @@
 """CPU: planarslam_b200/csrc/manhattan_body.h - the code the CUDA kernel k_track_manhattan runs, one thread per frame - compiled for
 the HOST with g++ and compared with the oracle (oracle/manhattan.cc, an independent statement with index lists and the generic
 Jacobi SVD).  Counts, found flags and membership masks must be identical, the rotation equal to float rounding.  The kernels
-themselves are checked on a B200 by tests/test_manhattan_gpu.py and tests/test_cuda_vs_reference_functions_gpu.py."""
+themselves are checked on an H100 by tests/test_manhattan_gpu.py and tests/test_cuda_vs_reference_functions_gpu.py."""
 import ctypes as C
 import os
 import subprocess

@@ -4,7 +4,7 @@ TrackManhattanFrame, map-line frustum test, ComputeStereoFromRGBD), run end to e
 The stand-in (tests/host_harness/mock_abi.cc) is built from the same shared host/device bodies the CUDA kernels call and includes
 include/pslam_abi.h, so its signatures are the real ABI's.  What this covers that the per-body host tests do not: argument order
 and dtypes of the ctypes calls, array shapes / padding of the batch forms, and the assertions of the GPU tests themselves - so that
-the first run on a B200 can only fail for a reason inside the kernels' launch code.  Test infrastructure only: the product library
+the first run on a GPU can only fail for a reason inside the kernels' launch code.  Test infrastructure only: the product library
 is not involved and keeps having no CPU path."""
 import ctypes as C
 import os

@@ -14,7 +14,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 N_BASE = 8
-BATCH = 1184
+BATCH = 1056           # 8 frames per SM of an H100 SXM (132 SMs)
 
 
 def lines3d_signature(out, drawn):
