@@ -33,7 +33,6 @@ struct LsdGeom {
     int refine;               // 0 NONE, 1 STD, 2 ADV
     int seg_cap;              // segment capacity per frame
     int cand_cap;             // candidate rectangles per frame (before the NFA validation)
-    int r2r_staged;           // region2rect: 1 = sums folded by three lanes over shared-memory staging (default), 0 = every lane folds through shuffles (PSLAM_LSD_R2R=shfl)
     int rect_enum;            // pixel enumeration of the NFA validation: 0 published LSD rectangle iterator, 1 cv2 4.x rect_nfa (lsd_rectenum.h)
     int min_reg_size;
     double rho, prec, p, log_nt, density_th, log_eps;
@@ -44,7 +43,7 @@ struct LsdGeom {
 // Per scaled pixel, three planes (k_lsd_gradient writes them, 16 bytes in all):
 //   ang  uint32  bits 0..30 = float bits of the level-line angle in degrees, fastAtan2(gx, -gy) (>= 0), or LSD_ANG_UNDEF (+inf) when the gradient norm is
 //                <= rho; bit 31 = the pixel belongs to a region ("used").  Region growing tests a neighbour with ONE 4-byte load; only k_lsd_regions writes it.
-//   cs   float2  cosf / sinf of the float angle (host-libm table indexed by (gx, gy)); read for accepted pixels only
+//   cs   float2  cosf / sinf of the float angle (host-libm table indexed by (gx, gy)); region growing reads it together with the angle word
 //   gxy  uint32  gx | gy << 16 (int16 each): gradient norm for the rectangle fit and the seed ordering
 #define LSD_ANG_UNDEF 0x7f800000u
 #define LSD_ANG_USED 0x80000000u
@@ -218,7 +217,6 @@ struct LsdFrame {                 // per-frame views
     uint32_t* ang;                // angle | used plane (see above); k_lsd_validate / k_lsd_improve only read it
     const float2* cs; const uint32_t* gxy;
     uint32_t* reg; uint32_t* order;
-    uint32_t* ring;               // shared memory: the last LSD_RING entries appended to reg[] (reg[i] lives in ring[i % LSD_RING])
     int W, H;
 };
 __device__ __forceinline__ bool lsd_word_used(uint32_t w) { return (w & LSD_ANG_USED) != 0; }
@@ -265,157 +263,96 @@ __device__ __forceinline__ double lsd_dist_sq(double x1, double y1, double x2, d
 // with the CURRENT region angle is taken, the angle is updated, and every lane that looks at the pixel just taken (another
 // group's overlapping neighbourhood) drops its candidate.  Entries appended during a step belong to later steps, exactly like
 // the reference's queue.  The records of the next step's neighbourhoods are requested one step ahead when the queue is long
-// enough; the `used` bytes are read at the start of a step (they depend on the previous step's acceptances).
-__device__ __forceinline__ uint32_t lsd_reg_read(const LsdFrame& F, int idx, int size) {
-    return size - idx <= LSD_RING ? F.ring[idx & (LSD_RING - 1)] : F.reg[idx];
-}
+// enough; the `used` bits are read at the start of a step (they depend on the previous step's acceptances).
+//
+// The serial chain of a step is the replay: ballot, shuffle of the winner's (cos, sin), float sums, atan2, alignment test.  Everything
+// else is kept off it: the (cos, sin) pair is loaded with the angle word (its address is known before the word arrives), and the
+// replay only records which lanes accepted - the used bit, the reg[] entry and the ring slot of every accepted pixel are written
+// after it by the accepting lanes at once (nothing in the step reads them; acceptances are in increasing lane order, so an
+// accepted lane's rank among the accepted lanes is its queue position).  The views are plain arguments so that they stay in registers.
+struct LsdGrown { double angle; int size; };
 template <int V>
-__device__ __noinline__ int lsd_region_grow(const LsdFrame& F, const LsdGeom& g, uint32_t seed, double prec, double& reg_angle_out) {
+__device__ __noinline__ LsdGrown lsd_region_grow(uint32_t* ang, const float2* __restrict__ cs, uint32_t* reg, int W, int H, uint32_t seed, double prec) {
+    __shared__ uint32_t ring[LSD_RING];           // the last LSD_RING entries appended to reg[] (reg[i] lives in ring[i % LSD_RING])
     const int lane = threadIdx.x & 31;
+    const unsigned below = (1u << lane) - 1u;
     const int q = lane >> 3, k8 = lane & 7;
     const int kk = k8 + (k8 >= 4);                 // index in the 3x3 window, centre skipped
     const int dyl = kk / 3 - 1, dxl = kk % 3 - 1;
     const int sx = seed & 0xffff, sy = seed >> 16;
-    const uint32_t ws = F.ang[(size_t)sy * F.W + sx];
+    const uint32_t ws = ang[(size_t)sy * W + sx];
     double reg_angle = lsd_word_angle(ws);
-    const double seed_angle = reg_angle;
-    float sumdx = 0.f, sumdy = 0.f;            // cos / sin of the seed angle: evaluated at the first acceptance (most seeds stay alone)
-    if (lane == 0) { F.reg[0] = seed; F.ring[0] = seed; F.ang[(size_t)sy * F.W + sx] = ws | LSD_ANG_USED; }
+    float sumdx = 0.f, sumdy = 0.f;
+    if (lane == 0) { reg[0] = seed; ring[0] = seed; ang[(size_t)sy * W + sx] = ws | LSD_ANG_USED; }
     __syncwarp();
+    // this lane's neighbour of queue entry idx: pixel, angle word and (cos, sin); out-of-image neighbours keep npix = ~0, LSD_ANG_UNDEF
+    auto probe = [&](int idx, int size, uint32_t& npix, uint32_t& w, float2& csv) {
+        const uint32_t pp = size - idx <= LSD_RING ? ring[idx & (LSD_RING - 1)] : reg[idx];
+        const int nx = (int)(pp & 0xffff) + dxl, ny = (int)(pp >> 16) + dyl;
+        if (nx >= 0 && ny >= 0 && nx < W && ny < H) {
+            const size_t o = (size_t)ny * W + nx;
+            w = ang[o]; csv = __ldg(cs + o); npix = (uint32_t)nx | ((uint32_t)ny << 16);
+        }
+    };
     int size = 1, i = 0;
     bool have_next = false;
     uint32_t np_next = 0xffffffffu, w_next = LSD_ANG_UNDEF;
+    float2 cs_next = make_float2(0.f, 0.f);
     while (true) {
         const int navail = min(4, size - i);
-        uint32_t npix, w;
-        if (have_next) { npix = np_next; w = w_next; }       // navail == 4; w_next was kept up to date while the previous step accepted pixels
-        else {
-            npix = 0xffffffffu; w = LSD_ANG_UNDEF;
-            if (q < navail) {
-                const uint32_t pp = lsd_reg_read(F, i + q, size);
-                const int nx = (int)(pp & 0xffff) + dxl, ny = (int)(pp >> 16) + dyl;
-                if (nx >= 0 && ny >= 0 && nx < F.W && ny < F.H) { w = F.ang[(size_t)ny * F.W + nx]; npix = (uint32_t)nx | ((uint32_t)ny << 16); }
-            }
-        }
+        uint32_t npix = 0xffffffffu, w = LSD_ANG_UNDEF;
+        float2 csv = make_float2(0.f, 0.f);
+        if (have_next) { npix = np_next; w = w_next; csv = cs_next; }     // navail == 4; w_next was kept up to date while the previous step accepted pixels
+        else if (q < navail) probe(i + q, size, npix, w, csv);
         // request the next step's neighbourhoods (entries i + 4 .. i + 7 exist already); acceptances of THIS step are patched into w_next below
         have_next = size - i >= 8;
-        np_next = 0xffffffffu; w_next = LSD_ANG_UNDEF;
-        if (have_next) {
-            const uint32_t pp = lsd_reg_read(F, i + 4 + q, size);
-            const int nx = (int)(pp & 0xffff) + dxl, ny = (int)(pp >> 16) + dyl;
-            if (nx >= 0 && ny >= 0 && nx < F.W && ny < F.H) { w_next = F.ang[(size_t)ny * F.W + nx]; np_next = (uint32_t)nx | ((uint32_t)ny << 16); }
-        }
+        np_next = 0xffffffffu; w_next = LSD_ANG_UNDEF; cs_next = make_float2(0.f, 0.f);
+        if (have_next) probe(i + 4 + q, size, np_next, w_next, cs_next);
         bool cand = lsd_word_defined(w) && !lsd_word_used(w);           // out-of-image lanes carry LSD_ANG_UNDEF
         const double a_n = lsd_word_angle(w);
-        // cos / sin of the candidates that are aligned right now (nearly every accepted pixel is): requested before the replay; the others load on demand
-        float2 csv = make_float2(0.f, 0.f);
-        bool have_cs = cand && lsd_aligned_angle(a_n, reg_angle, prec);
-        if (have_cs) csv = __ldg(F.cs + (size_t)(npix >> 16) * F.W + (npix & 0xffff));
+        // cos / sin of the seed angle start the sums; evaluated only when the seed's first step accepts a pixel (most seeds stay alone)
+        if (size == 1 && __any_sync(0xffffffffu, cand && lsd_aligned_angle(a_n, reg_angle, prec))) {
+            double sn0, cs0;
+            lsd_sincos<V>(reg_angle, sn0, cs0);
+            sumdx = (float)cs0; sumdy = (float)sn0;
+        }
         int last = -1;
+        unsigned taken = 0;
         while (true) {
             const bool al = cand && lane > last && lsd_aligned_angle(a_n, reg_angle, prec);
             const unsigned m = __ballot_sync(0xffffffffu, al);
             if (!m) break;
             const int j = __ffs(m) - 1;
-            if (lane == j) {
-                if (!have_cs) { csv = __ldg(F.cs + (size_t)(npix >> 16) * F.W + (npix & 0xffff)); have_cs = true; }
-                F.ang[(size_t)(npix >> 16) * F.W + (npix & 0xffff)] = w | LSD_ANG_USED;
-                F.reg[size] = npix; F.ring[size & (LSD_RING - 1)] = npix;
-            }
             const float cj = __shfl_sync(0xffffffffu, csv.x, j), sj = __shfl_sync(0xffffffffu, csv.y, j);
             const uint32_t np = __shfl_sync(0xffffffffu, npix, j);
-            if (size == 1) { double sn0, cs0; lsd_sincos<V>(seed_angle, sn0, cs0); sumdx = (float)cs0; sumdy = (float)sn0; }
             sumdx = __fadd_rn(sumdx, cj);
             sumdy = __fadd_rn(sumdy, sj);
             reg_angle = (double)lsd_fast_atan2_deg(sumdy, sumdx) * LSD_DEG2RAD;
             if (npix == np) cand = false;                  // the pixel is used now (lane j itself and overlapping neighbourhoods of the other groups)
             if (np_next == np) w_next |= LSD_ANG_USED;     // ... and in the neighbourhoods already requested for the next step
-            ++size;
+            taken |= 1u << j;
             last = j;
         }
+        if (taken >> lane & 1u) {
+            const int at = size + __popc(taken & below);
+            ang[(size_t)(npix >> 16) * W + (npix & 0xffff)] = w | LSD_ANG_USED;
+            reg[at] = npix; ring[at & (LSD_RING - 1)] = npix;
+        }
+        size += __popc(taken);
         __syncwarp();
         i += navail;
         if (i >= size) break;
     }
-    reg_angle_out = reg_angle;
-    return size;
-}
-
-// In-order double sums over the region (region2rect + get_theta).  Lanes load 32 entries at a time; every lane accumulates
-// the whole sequence, so the result is the sequential sum and is uniform across the warp.
-template <int V>
-__device__ __noinline__ void lsd_region2rect_shfl(const LsdFrame& F, int size, double reg_angle, double prec, double p, LsdRect& rec) {
-    const int lane = threadIdx.x & 31;
-    double x = 0, y = 0, sum = 0;
-    for (int base = 0; base < size; base += 32) {
-        int mx = 0, my = 0; double mw = 0;
-        if (base + lane < size) {
-            const uint32_t pp = F.reg[base + lane];
-            mx = pp & 0xffff; my = pp >> 16;
-            mw = lsd_pix_norm(F, mx, my);
-        }
-        const int cnt = min(32, size - base);
-        for (int t = 0; t < cnt; ++t) {
-            const double w = __shfl_sync(0xffffffffu, mw, t);
-            const int px = __shfl_sync(0xffffffffu, mx, t), py = __shfl_sync(0xffffffffu, my, t);
-            x += (double)px * w;
-            y += (double)py * w;
-            sum += w;
-        }
-    }
-    x /= sum;
-    y /= sum;
-    double Ixx = 0.0, Iyy = 0.0, Ixy = 0.0;
-    for (int base = 0; base < size; base += 32) {
-        int mx = 0, my = 0; double mw = 0;
-        if (base + lane < size) {
-            const uint32_t pp = F.reg[base + lane];
-            mx = pp & 0xffff; my = pp >> 16;
-            mw = lsd_pix_norm(F, mx, my);
-        }
-        const int cnt = min(32, size - base);
-        for (int t = 0; t < cnt; ++t) {
-            const double w = __shfl_sync(0xffffffffu, mw, t);
-            const double ddx = (double)__shfl_sync(0xffffffffu, mx, t) - x, ddy = (double)__shfl_sync(0xffffffffu, my, t) - y;
-            Ixx += ddy * ddy * w;
-            Iyy += ddx * ddx * w;
-            Ixy -= ddx * ddy * w;
-        }
-    }
-    const double lambda = 0.5 * (Ixx + Iyy - sqrt((Ixx - Iyy) * (Ixx - Iyy) + 4.0 * Ixy * Ixy));
-    double theta = (fabs(Ixx) > fabs(Iyy)) ? (double)lsd_fast_atan2_deg((float)(lambda - Ixx), (float)Ixy) : (double)lsd_fast_atan2_deg((float)Ixy, (float)(lambda - Iyy));
-    theta *= LSD_DEG2RAD;
-    if (fabs(lsd_angle_diff_signed(theta, reg_angle)) > prec) theta += LSD_PI;
-    double dx, dy;
-    lsd_sincos<V>(theta, dy, dx);
-    double l_min = 0, l_max = 0, w_min = 0, w_max = 0;
-    for (int base = 0; base < size; base += 32) {
-        int mx = 0, my = 0;
-        if (base + lane < size) { const uint32_t pp = F.reg[base + lane]; mx = pp & 0xffff; my = pp >> 16; }
-        const int cnt = min(32, size - base);
-        for (int t = 0; t < cnt; ++t) {
-            const double regdx = (double)__shfl_sync(0xffffffffu, mx, t) - x, regdy = (double)__shfl_sync(0xffffffffu, my, t) - y;
-            const double l = regdx * dx + regdy * dy;
-            const double w = -regdx * dy + regdy * dx;
-            if (l > l_max) l_max = l; else if (l < l_min) l_min = l;
-            if (w > w_max) w_max = w; else if (w < w_min) w_min = w;
-        }
-    }
-    rec.x1 = x + l_min * dx; rec.y1 = y + l_min * dy;
-    rec.x2 = x + l_max * dx; rec.y2 = y + l_max * dy;
-    rec.width = w_max - w_min;
-    rec.x = x; rec.y = y; rec.theta = theta; rec.dx = dx; rec.dy = dy; rec.prec = prec; rec.p = p;
-    if (rec.width < 1.0) rec.width = 1.0;
+    return {reg_angle, size};
 }
 
 // region2rect + get_theta with the order-sensitive part reduced to its minimum.  The reference's running sums are sequential double additions; what is added - the
 // products x * w, (dy * dy) * w ... - does not depend on the order.  So the lanes compute the terms of 32 region points at once and park them in shared memory, and
 // lanes 0, 1, 2 each fold one of the three sums in point order (one shared-memory load + one DADD per point for all three sums together, instead of four
 // shuffles and five to nine double operations per point in every lane).  The extent pass is a plain min / max: l_max >= 0 >= l_min always hold (both start at 0),
-// so the reference's "else if" never skips an update and the order is irrelevant.  Bit-identical to lsd_region2rect_shfl (the round-2 version, kept selectable).
+// so the reference's "else if" never skips an update and the order is irrelevant.
 template <int V>
-__device__ __noinline__ void lsd_region2rect(const LsdFrame& F, const LsdGeom& g, int size, double reg_angle, double prec, double p, LsdRect& rec) {
-    if (!g.r2r_staged) { lsd_region2rect_shfl<V>(F, size, reg_angle, prec, p, rec); return; }
+__device__ __noinline__ void lsd_region2rect(const LsdFrame& F, int size, double reg_angle, double prec, double p, LsdRect& rec) {
     __shared__ double s_stage[96];                                      // [3][32] terms of the three running sums (the CTA is one warp)
     const int lane = threadIdx.x & 31;
     const double* const mine = s_stage + 32 * (lane < 3 ? lane : 2);    // the sum this lane folds (lanes above 2 fold a copy that is never read)
@@ -485,64 +422,95 @@ __device__ __forceinline__ double lsd_density(int size, const LsdRect& rec) {
 }
 
 // LineSegmentDetectorImpl::refine + reduce_region_radius; returns false when the region is dropped.  size / reg_angle / rec updated.
+// The angle statistics are warp-parallel like lsd_region2rect: every lane computes the terms of its point (0 for the points outside the radius: the sums start
+// at +0 and never become -0, so adding +0 leaves them unchanged) and lanes 0, 1 fold the two sums in point order over shared-memory staging.
 template <int V>
 __device__ __noinline__ bool lsd_refine(const LsdFrame& F, const LsdGeom& g, int& size, double& reg_angle, LsdRect& rec) {
+    __shared__ double s_ang[64];                                        // [2][32] terms of sum and s_sum
     const int lane = threadIdx.x & 31;
+    const unsigned below = (1u << lane) - 1u;
     double density = lsd_density(size, rec);
     if (density >= g.density_th) return true;
-    const uint32_t p0 = F.reg[0];
+    uint32_t* const ang = F.ang;
+    uint32_t* const reg = F.reg;
+    const int W = F.W;
+    const uint32_t p0 = reg[0];
     const double xc = (double)(p0 & 0xffff), yc = (double)(p0 >> 16);
-    const double ang_c = lsd_word_angle(F.ang[(size_t)(p0 >> 16) * F.W + (p0 & 0xffff)]);
-    double sum = 0, s_sum = 0;
+    const double ang_c = lsd_word_angle(ang[(size_t)(p0 >> 16) * W + (p0 & 0xffff)]);
+    const double* const mine = s_ang + 32 * (lane & 1);
+    double acc = 0;
     int n = 0;
     for (int base = 0; base < size; base += 32) {
-        int mx = 0, my = 0; double ma = 0;
+        bool near = false;
         if (base + lane < size) {
-            const uint32_t pp = F.reg[base + lane];
-            mx = pp & 0xffff; my = pp >> 16;
-            const uint32_t wv = F.ang[(size_t)my * F.W + mx];
-            F.ang[(size_t)my * F.W + mx] = wv & 0x7fffffffu;           // used = NOTUSED for the whole region (every lane owns distinct pixels)
-            ma = lsd_word_angle(wv);
+            const uint32_t pp = reg[base + lane];
+            const int mx = pp & 0xffff, my = pp >> 16;
+            const uint32_t wv = ang[(size_t)my * W + mx];
+            ang[(size_t)my * W + mx] = wv & 0x7fffffffu;               // used = NOTUSED for the whole region (every lane owns distinct pixels)
+            double ang_d = 0;
+            near = sqrt(lsd_dist_sq(xc, yc, (double)mx, (double)my)) < rec.width;
+            if (near) ang_d = lsd_angle_diff_signed(lsd_word_angle(wv), ang_c);
+            s_ang[lane] = ang_d; s_ang[32 + lane] = ang_d * ang_d;
         }
+        n += __popc(__ballot_sync(0xffffffffu, near));
+        __syncwarp();
         const int cnt = min(32, size - base);
-        for (int t = 0; t < cnt; ++t) {
-            const double a = __shfl_sync(0xffffffffu, ma, t);
-            const double px = (double)__shfl_sync(0xffffffffu, mx, t), py = (double)__shfl_sync(0xffffffffu, my, t);
-            if (sqrt(lsd_dist_sq(xc, yc, px, py)) < rec.width) {
-                const double ang_d = lsd_angle_diff_signed(a, ang_c);
-                sum += ang_d;
-                s_sum += ang_d * ang_d;
-                ++n;
-            }
-        }
+        for (int t = 0; t < cnt; ++t) acc += mine[t];
+        __syncwarp();
     }
-    __syncwarp();
+    const double sum = __shfl_sync(0xffffffffu, acc, 0), s_sum = __shfl_sync(0xffffffffu, acc, 1);
     const double mean_angle = sum / (double)n;
     const double tau = 2.0 * sqrt((s_sum - 2.0 * mean_angle * sum) / (double)n + mean_angle * mean_angle);
-    size = lsd_region_grow<V>(F, g, p0, tau, reg_angle);
+    const LsdGrown gr = lsd_region_grow<V>(ang, F.cs, reg, W, F.H, p0, tau);
+    size = gr.size; reg_angle = gr.angle;
     if (size < 2) return false;
-    lsd_region2rect<V>(F, g, size, reg_angle, g.prec, g.p, rec);
+    lsd_region2rect<V>(F, size, reg_angle, g.prec, g.p, rec);
     density = lsd_density(size, rec);
     if (density >= g.density_th) return true;
-    // reduce_region_radius
+    // reduce_region_radius.  The reference walks reg[] once per radius, replacing every point farther than the radius by the last point (re-examined in its
+    // place) and shrinking the region.  That leaves the m = size - (far points) near points in reg[0 .. m): the near points below m stay where they are, and the
+    // k-th far point below m (in index order) is replaced by the k-th near point at or above m (in DESCENDING index order).  Three ballot passes build the same
+    // order: count the far points (and clear their used bits), pack the near points of reg[m .. size) against the end of the array in descending order, and fill
+    // the holes below m from there.  (The far points the reference parks in reg[m .. size) are not kept: nothing reads past the region.)
     double radSq1 = lsd_dist_sq(xc, yc, rec.x1, rec.y1), radSq2 = lsd_dist_sq(xc, yc, rec.x2, rec.y2);
     double radSq = radSq1 > radSq2 ? radSq1 : radSq2;
     while (density < g.density_th) {
         radSq *= 0.75 * 0.75;
-        for (int i = 0; i < size; ++i) {                    // swap-with-last removal, sequential like the reference
-            const uint32_t pp = F.reg[i];
-            const double px = (double)(pp & 0xffff), py = (double)(pp >> 16);
-            if (lsd_dist_sq(xc, yc, px, py) > radSq) {
-                const uint32_t lastp = F.reg[size - 1];
-                __syncwarp();
-                if (lane == 0) { F.ang[(size_t)(pp >> 16) * F.W + (pp & 0xffff)] &= 0x7fffffffu; F.reg[i] = lastp; F.reg[size - 1] = pp; }
-                __syncwarp();
-                --size;
-                --i;
+        auto far_point = [&](uint32_t pp) { return lsd_dist_sq(xc, yc, (double)(pp & 0xffff), (double)(pp >> 16)) > radSq; };
+        int nfar = 0;
+        for (int base = 0; base < size; base += 32) {
+            bool f = false;
+            if (base + lane < size) {
+                const uint32_t pp = reg[base + lane];
+                f = far_point(pp);
+                if (f) ang[(size_t)(pp >> 16) * W + (pp & 0xffff)] &= 0x7fffffffu;
             }
+            nfar += __popc(__ballot_sync(0xffffffffu, f));
         }
+        const int m = size - nfar;
+        int r = 0;
+        for (int top = size - 1; top >= m; top -= 32) {          // lane t reads reg[top - t]; every write lands at or above the index its lane read
+            const int idx = top - lane;
+            uint32_t pp = 0;
+            bool keep = false;
+            if (idx >= m) { pp = reg[idx]; keep = !far_point(pp); }
+            const unsigned k = __ballot_sync(0xffffffffu, keep);
+            if (keep) reg[size - 1 - (r + __popc(k & below))] = pp;
+            r += __popc(k);
+        }
+        __syncwarp();
+        r = 0;
+        for (int base = 0; base < m; base += 32) {
+            const int idx = base + lane;
+            const bool hole = idx < m && far_point(reg[idx]);
+            const unsigned h = __ballot_sync(0xffffffffu, hole);
+            if (hole) reg[idx] = reg[size - 1 - (r + __popc(h & below))];
+            r += __popc(h);
+        }
+        __syncwarp();
+        size = m;
         if (size < 2) return false;
-        lsd_region2rect<V>(F, g, size, reg_angle, g.prec, g.p, rec);
+        lsd_region2rect<V>(F, size, reg_angle, g.prec, g.p, rec);
         density = lsd_density(size, rec);
     }
     return true;
@@ -810,7 +778,6 @@ __global__ void __launch_bounds__(32, V) k_lsd_regions(LsdGeom g, int nframes, u
                                                     const int32_t* __restrict__ smax, uint32_t* __restrict__ reg_all, const uint32_t* __restrict__ order_all,
                                                     const int32_t* __restrict__ n_order, double* __restrict__ cands, int32_t* __restrict__ n_cand,
                                                     int32_t* __restrict__ status) {
-    __shared__ uint32_t s_ring[LSD_RING];
     const int lane = threadIdx.x & 31;
     const int frame = blockIdx.x;
     if (frame >= nframes) return;
@@ -818,7 +785,6 @@ __global__ void __launch_bounds__(32, V) k_lsd_regions(LsdGeom g, int nframes, u
     LsdFrame F;
     F.ang = ang_all + (size_t)frame * npx; F.cs = cs_all + (size_t)frame * npx; F.gxy = gxy_all + (size_t)frame * npx; F.reg = reg_all + (size_t)frame * npx;
     F.order = const_cast<uint32_t*>(order_all) + (size_t)frame * npx; F.W = g.W; F.H = g.H;
-    F.ring = s_ring;
     int count_out = 0;
     const int n_def = smax[frame] > 0 ? n_order[frame] : 0;
     {
@@ -834,11 +800,12 @@ __global__ void __launch_bounds__(32, V) k_lsd_regions(LsdGeom g, int nframes, u
                 const int j = __ffs(m) - 1;
                 last = j;
                 const uint32_t seed = __shfl_sync(0xffffffffu, mypix, j);
-                double reg_angle;
-                int size = lsd_region_grow<V>(F, g, seed, g.prec, reg_angle);
+                const LsdGrown gr = lsd_region_grow<V>(F.ang, F.cs, F.reg, F.W, F.H, seed, g.prec);
+                int size = gr.size;
+                double reg_angle = gr.angle;
                 if (size < g.min_reg_size) continue;
                 LsdRect rc;
-                lsd_region2rect<V>(F, g, size, reg_angle, g.prec, g.p, rc);
+                lsd_region2rect<V>(F, size, reg_angle, g.prec, g.p, rc);
                 if (g.refine > 0 && !lsd_refine<V>(F, g, size, reg_angle, rc)) continue;
                 // candidate rectangle, in detection order; the NFA validation / improvement of LSD_REFINE_ADV does not touch
                 // the 'used' map, so it runs afterwards with one thread per candidate (k_lsd_validate)
@@ -873,7 +840,7 @@ __global__ void __launch_bounds__(64) k_lsd_validate(LsdGeom g, const uint32_t* 
     const int n = min(n_cand[frame], g.cand_cap);
     if (ci >= n) return;
     LsdFrame F;
-    F.ang = const_cast<uint32_t*>(ang_all) + (size_t)frame * g.W * g.H; F.cs = nullptr; F.gxy = nullptr; F.reg = nullptr; F.order = nullptr; F.ring = nullptr; F.W = g.W; F.H = g.H;
+    F.ang = const_cast<uint32_t*>(ang_all) + (size_t)frame * g.W * g.H; F.cs = nullptr; F.gxy = nullptr; F.reg = nullptr; F.order = nullptr; F.W = g.W; F.H = g.H;
     LsdRect rc;
     lsd_load_cand(cands + ((size_t)frame * g.cand_cap + ci) * 12, rc);
     const double log_nfa = lsd_rect_nfa_scalar(F, g, rc);
@@ -887,7 +854,7 @@ __global__ void __launch_bounds__(64) k_lsd_improve(LsdGeom g, const uint32_t* _
     if (k >= n_fail[frame]) return;
     const int ci = (int)fail_list[(size_t)frame * g.cand_cap + k];
     LsdFrame F;
-    F.ang = const_cast<uint32_t*>(ang_all) + (size_t)frame * g.W * g.H; F.cs = nullptr; F.gxy = nullptr; F.reg = nullptr; F.order = nullptr; F.ring = nullptr; F.W = g.W; F.H = g.H;
+    F.ang = const_cast<uint32_t*>(ang_all) + (size_t)frame * g.W * g.H; F.cs = nullptr; F.gxy = nullptr; F.reg = nullptr; F.order = nullptr; F.W = g.W; F.H = g.H;
     double* c = cands + ((size_t)frame * g.cand_cap + ci) * 12;
     LsdRect rc;
     lsd_load_cand(c, rc);

@@ -63,7 +63,6 @@ int lsd_alloc(pslam_ctx* c) {
         // or pslam_lsd_set_rect_enumeration(ctx, 0) select the published LSD iterator
         const char* e = std::getenv("PSLAM_LSD_RECT_ENUM");
         g.rect_enum = (e && (!std::strcmp(e, "published") || !std::strcmp(e, "0"))) ? 0 : 1;
-        { const char* r = std::getenv("PSLAM_LSD_R2R"); g.r2r_staged = (r && (!std::strcmp(r, "shfl") || !std::strcmp(r, "0"))) ? 0 : 1; }
     }
     g.prec = LSD_PI * ANG_TH / 180; g.p = ANG_TH / 180; g.rho = QUANT / std::sin(g.prec);
     g.log_nt = 5 * (std::log10(double(g.W)) + std::log10(double(g.H))) / 2 + std::log10(11.0);
