@@ -38,7 +38,7 @@ struct TrackBuffers {
     int32_t *d_cell_start = nullptr, *d_items = nullptr, *d_cand_n = nullptr, *d_scalar = nullptr, *d_hist_idx = nullptr; uint32_t* d_cand = nullptr;
     int8_t* d_hist_bin = nullptr; uint8_t* d_in_view = nullptr; size_t cap_pts = 0;
     // pose problem
-    PoseHeaderDev* d_hdr = nullptr; PoseEdgeDev* d_edges = nullptr; double* d_err = nullptr; uint8_t* d_level = nullptr; uint8_t* d_flags = nullptr;
+    PoseHeaderDev* d_hdr = nullptr; float4* d_pa = nullptr; float4* d_pb = nullptr; uint8_t* d_level = nullptr; uint8_t* d_flags = nullptr;
     PoseOutDev* d_out = nullptr; int32_t* d_kp_of_edge = nullptr; float* d_inv_sigma2 = nullptr;
     // per-frame outputs
     float* d_T_all = nullptr; int32_t* d_stats = nullptr;      // [n][16], [n][4] = matches / inliers after the motion-model stage and after the local-map stage
@@ -97,8 +97,8 @@ __global__ void k_track_fill(int32_t* __restrict__ a, int n, int32_t v) {
 // monocular when mvuRight[i] < 0, stereo otherwise; information = mvInvLevelSigma2[octave]; Huber deltas sqrt(5.991) / sqrt(7.815) as float.
 __global__ void __launch_bounds__(256) k_track_pack(const pslam_keypoint* __restrict__ keys, const float* __restrict__ u_right, const int32_t* __restrict__ n_kp, int cap,
                                                     const int32_t* __restrict__ matches, const float* __restrict__ map_pos, const float* __restrict__ inv_sigma2,
-                                                    TrackCam K, const float* __restrict__ Tcw, PoseHeaderDev* __restrict__ hdr, PoseEdgeDev* __restrict__ edges,
-                                                    int32_t* __restrict__ kp_of_edge) {
+                                                    TrackCam K, const float* __restrict__ Tcw, PoseHeaderDev* __restrict__ hdr, float4* __restrict__ pt_a,
+                                                    float4* __restrict__ pt_b, int32_t* __restrict__ kp_of_edge) {
     __shared__ int s_part[256];
     const int tid = threadIdx.x;
     const int n = min(*n_kp, cap);
@@ -123,18 +123,11 @@ __global__ void __launch_bounds__(256) k_track_pack(const pslam_keypoint* __rest
     for (int i = b0; i < b1; ++i) {
         const int m = matches[i];
         if (m < 0) continue;
-        PoseEdgeDev e;
-        memset(&e, 0, sizeof e);
         const float ur = u_right[i];
         const bool mono = ur < 0;
-        e.kind = mono ? PK_MONO : PK_STEREO; e.idx = pos;
         const pslam_keypoint kp = keys[i];
-        e.a[0] = (double)map_pos[3 * m]; e.a[1] = (double)map_pos[3 * m + 1]; e.a[2] = (double)map_pos[3 * m + 2];
-        e.a[3] = (double)kp.x; e.a[4] = (double)kp.y; e.a[5] = (double)ur;
-        const double w = (double)inv_sigma2[kp.octave];
-        e.info[0] = w; e.info[1] = w; e.info[2] = w;
-        e.delta = (double)(mono ? deltaMono : deltaStereo);
-        edges[pos] = e;
+        pt_a[pos] = make_float4(map_pos[3 * m], map_pos[3 * m + 1], map_pos[3 * m + 2], kp.x);     // the point record of pose_kernels.cuh
+        pt_b[pos] = make_float4(kp.y, ur, inv_sigma2[kp.octave], mono ? deltaMono : deltaStereo);
         kp_of_edge[pos] = i;
         ++pos;
     }
@@ -156,7 +149,7 @@ __global__ void __launch_bounds__(256) k_track_sweep(const PoseHeaderDev* __rest
 static void track_free_buffers(TrackBuffers& B) {
     for (void* p : {B.map_blob, (void*)B.d_skip, (void*)B.d_skip0, (void*)B.d_kps, (void*)B.d_desc, (void*)B.d_n, (void*)B.d_ur, (void*)B.d_dz, (void*)B.d_T, (void*)B.d_matches,
                     (void*)B.d_zero, (void*)B.d_cell_start, (void*)B.d_items, (void*)B.d_cand_n, (void*)B.d_scalar, (void*)B.d_hist_idx, (void*)B.d_cand, (void*)B.d_hist_bin,
-                    (void*)B.d_in_view, (void*)B.d_hdr, (void*)B.d_edges, (void*)B.d_err, (void*)B.d_level, (void*)B.d_flags, (void*)B.d_out, (void*)B.d_kp_of_edge,
+                    (void*)B.d_in_view, (void*)B.d_hdr, (void*)B.d_pa, (void*)B.d_pb, (void*)B.d_level, (void*)B.d_flags, (void*)B.d_out, (void*)B.d_kp_of_edge,
                     (void*)B.d_inv_sigma2, (void*)B.d_T_all, (void*)B.d_stats})
         if (p) cudaFree(p);
 }
@@ -226,7 +219,7 @@ int pslam_track_sequence_dev(pslam_ctx* c, const uint8_t* d_gray, const uint16_t
     }
     if (cap != B.cap) {
         TA(B.d_T, 3 * 64); TA(B.d_matches, (size_t)2 * cap * 4); TA(B.d_zero, cap); TA(B.d_cell_start, (SG_CELLS + 1) * 4); TA(B.d_items, SEARCH_MAX_KP * 4);
-        TA(B.d_scalar, 16); TA(B.d_hdr, sizeof(PoseHeaderDev)); TA(B.d_edges, (size_t)cap * sizeof(PoseEdgeDev)); TA(B.d_err, (size_t)cap * 24); TA(B.d_level, cap);
+        TA(B.d_scalar, 16); TA(B.d_hdr, sizeof(PoseHeaderDev)); TA(B.d_pa, (size_t)cap * sizeof(float4)); TA(B.d_pb, (size_t)cap * sizeof(float4)); TA(B.d_level, cap);
         TA(B.d_flags, cap); TA(B.d_out, sizeof(PoseOutDev)); TA(B.d_kp_of_edge, (size_t)cap * 4); TA(B.d_inv_sigma2, PSLAM_MAX_LEVELS * 4);
         PSLAM_CUDA(c, cudaMemsetAsync(B.d_zero, 0, cap, st));
         PSLAM_CUDA(c, cudaMemcpyAsync(B.d_inv_sigma2, c->inv_sigma2.data(), g.nlevels * 4, cudaMemcpyHostToDevice, st));
@@ -257,10 +250,10 @@ int pslam_track_sequence_dev(pslam_ctx* c, const uint8_t* d_gray, const uint16_t
     const TrackCam K{prm->fx, prm->fy, prm->cx, prm->cy, prm->bf};
     int32_t* m_cur = B.d_matches; int32_t* m_last = B.d_matches + cap;
     auto optimise = [&](int t, int stage) -> int {
-        PSLAM_LAUNCH(c, "track_pack", k_track_pack<<<1, 256, 0, st>>>(F.keys_un, F.u_right, F.n_dev, cap, m_cur, B.M.pos, B.d_inv_sigma2, K, B.d_T, B.d_hdr, B.d_edges,
-                     B.d_kp_of_edge));
-        PSLAM_LAUNCH(c, "pose_optimization", k_pose_optimization<<<1, POSE_THREADS, 0, st>>>(B.d_hdr, B.d_edges, B.d_err, B.d_level, B.d_flags, B.d_flags, B.d_flags,
-                     B.d_flags, B.d_flags, B.d_out));
+        PSLAM_LAUNCH(c, "track_pack", k_track_pack<<<1, 256, 0, st>>>(F.keys_un, F.u_right, F.n_dev, cap, m_cur, B.M.pos, B.d_inv_sigma2, K, B.d_T, B.d_hdr, B.d_pa,
+                     B.d_pb, B.d_kp_of_edge));
+        PSLAM_LAUNCH(c, "pose_optimization", k_pose_optimization<<<1, POSE_THREADS, 0, st>>>(B.d_hdr, B.d_pa, B.d_pb, nullptr, nullptr, B.d_level, B.d_flags,
+                     B.d_flags, B.d_flags, B.d_flags, B.d_flags, B.d_out));
         PSLAM_LAUNCH(c, "track_sweep", k_track_sweep<<<1, 256, 0, st>>>(B.d_hdr, B.d_out, B.d_flags, B.d_kp_of_edge, m_cur, B.d_T, B.d_stats + 4 * t + 2 * stage));
         return PSLAM_OK;
     };
