@@ -12,7 +12,8 @@
 //                      region points are evaluated by the 32 lanes, acceptances are replayed in order because every accepted pixel
 //                      moves the region angle), rectangle fit with in-order double sums, density refinement; emits candidate
 //                      rectangles; latency-bound
-//   k_lsd_validate     one thread per candidate: first NFA evaluation (log-gamma from a host-built table), failures queued;
+//   k_lsd_validate     one thread per candidate: first NFA evaluation (aligned pixels counted on integer word intervals, lsd_alignbounds.h; the NFA
+//                      from a per-context table built on the device), failures queued;
 //   k_lsd_improve      one thread per queued candidate: the remaining rect_improve stages; k_lsd_emit compacts
 //   k_lsd_keylines     the 40 longest segments -> cv::line_descriptor::KeyLine records + line functions
 #pragma once
@@ -21,6 +22,7 @@
 #include <cfloat>
 #include <cstdint>
 
+#include "lsd_alignbounds.h"
 #include "lsd_detsincos.h"
 #include "lsd_rectenum.h"
 #include "pslam_internal.h"
@@ -37,6 +39,7 @@ struct LsdGeom {
     int min_reg_size;
     double rho, prec, p, log_nt, density_th, log_eps;
     const double* lgamma_tab;  // log_gamma(i) for i = 0 .. LSD_LGAMMA_N - 1, evaluated by the host with the reference's formulas
+    const double* nfa_tab;     // NFA(n, k, p / 2^j) for n <= LSD_NFA_NMAX, j < LSD_NFA_NJ (lsd_nfa), built on the device by k_lsd_nfa_table
 };
 #define LSD_LGAMMA_N 8192
 
@@ -45,13 +48,9 @@ struct LsdGeom {
 //                <= rho; bit 31 = the pixel belongs to a region ("used").  Region growing tests a neighbour with ONE 4-byte load; only k_lsd_regions writes it.
 //   cs   float2  cosf / sinf of the float angle (host-libm table indexed by (gx, gy)); region growing reads it together with the angle word
 //   gxy  uint32  gx | gy << 16 (int16 each): gradient norm for the rectangle fit and the seed ordering
-#define LSD_ANG_UNDEF 0x7f800000u
+// (LSD_ANG_UNDEF, the angle constants, lsd_word_angle and lsd_aligned_angle live in lsd_alignbounds.h)
 #define LSD_ANG_USED 0x80000000u
 
-#define LSD_PI 3.14159265358979323846
-#define LSD_DEG2RAD (LSD_PI / 180)
-#define LSD_3_2_PI ((3 * LSD_PI) / 2)
-#define LSD_2PI (2 * LSD_PI)
 #define LSD_LN10 2.30258509299404568402
 
 __device__ __forceinline__ float lsd_fast_atan2_deg(float y, float x) {       // cv::fastAtan2 (same arithmetic as the ORB path)
@@ -221,21 +220,9 @@ struct LsdFrame {                 // per-frame views
 };
 __device__ __forceinline__ bool lsd_word_used(uint32_t w) { return (w & LSD_ANG_USED) != 0; }
 __device__ __forceinline__ bool lsd_word_defined(uint32_t w) { return (w & 0x7fffffffu) < LSD_ANG_UNDEF; }
-__device__ __forceinline__ float lsd_word_deg(uint32_t w) { return __uint_as_float(w & 0x7fffffffu); }
-__device__ __forceinline__ double lsd_word_angle(uint32_t w) { return (double)lsd_word_deg(w) * LSD_DEG2RAD; }
 __device__ __forceinline__ double lsd_pix_norm(const LsdFrame& F, int x, int y) {
     const uint32_t v = __ldg(F.gxy + (size_t)y * F.W + x);
     return lsd_norm((int)(short)(v & 0xffff), (int)(short)(v >> 16));
-}
-
-__device__ __forceinline__ bool lsd_aligned_angle(double a, double theta, double prec) {
-    double n_theta = theta - a;
-    if (n_theta < 0) n_theta = -n_theta;
-    if (n_theta > LSD_3_2_PI) {
-        n_theta -= LSD_2PI;
-        if (n_theta < 0) n_theta = -n_theta;
-    }
-    return n_theta <= prec;
 }
 
 __device__ __forceinline__ double lsd_angle_diff_signed(double a, double b) {
@@ -557,6 +544,31 @@ __device__ __noinline__ double lsd_nfa_scalar(int n, int k, double p, double log
     return -log10(bin_tail) - log_nt;
 }
 
+// The validation evaluates the NFA at p = g.p / 2^j only (rect_improve halves p, exactly, at most ten times) and mostly at small n (on the benchmark's frames
+// 99.998 % of the calls have n <= 512, the median is 19).  lsd_alloc therefore tabulates lsd_nfa_scalar itself, on the device, for every k <= n <= LSD_NFA_NMAX
+// and j < LSD_NFA_NJ: a lookup returns the very double the scalar evaluation gives.  Other arguments fall back to lsd_nfa_scalar.
+#define LSD_NFA_NMAX 512
+#define LSD_NFA_NJ 11
+#define LSD_NFA_TRI ((LSD_NFA_NMAX + 1) * (LSD_NFA_NMAX + 2) / 2)      // entries per j, at tri(n) + k with tri(n) = n (n + 1) / 2
+__global__ void __launch_bounds__(256) k_lsd_nfa_table(LsdGeom g, double* __restrict__ tab) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= LSD_NFA_NJ * LSD_NFA_TRI) return;
+    const int j = i / LSD_NFA_TRI, e = i - j * LSD_NFA_TRI;
+    int n = (int)((sqrt(8.0 * e + 1.0) - 1.0) / 2.0);
+    while (n * (n + 1) / 2 > e) --n;
+    while ((n + 1) * (n + 2) / 2 <= e) ++n;
+    double p = g.p;
+    for (int t = 0; t < j; ++t) p /= 2;
+    tab[i] = lsd_nfa_scalar(n, e - n * (n + 1) / 2, p, g.log_nt, g.lgamma_tab);
+}
+__device__ __forceinline__ double lsd_nfa(int n, int k, double p, const LsdGeom& g) {
+    if (n <= LSD_NFA_NMAX) {
+        const int j = ilogb(g.p) - ilogb(p);
+        if (j >= 0 && j < LSD_NFA_NJ && p == ldexp(g.p, -j)) return __ldg(g.nfa_tab + j * LSD_NFA_TRI + n * (n + 1) / 2 + k);
+    }
+    return lsd_nfa_scalar(n, k, p, g.log_nt, g.lgamma_tab);
+}
+
 __device__ __forceinline__ double lsd_inter_low(double x, double x1, double y1, double x2, double y2) {
     if (lsd_double_equal(x1, x2) && y1 < y2) return y1;
     if (lsd_double_equal(x1, x2) && y1 > y2) return y2;
@@ -569,7 +581,7 @@ __device__ __forceinline__ double lsd_inter_hi(double x, double x1, double y1, d
 }
 
 // Point counts of the published LSD rectangle iterator for rectangle r: this lane visits the columns xa + sub, xa + sub + stride, ...
-__device__ __forceinline__ void lsd_rect_count(const LsdFrame& F, const LsdGeom& g, const LsdRect& r, int sub, int stride, int& n, int& k) {
+__device__ __forceinline__ void lsd_rect_count(const LsdFrame& F, const LsdRect& r, const LsdAlignSet& S, int sub, int stride, int& n, int& k) {
     double vx[4], vy[4], rx[4], ry[4];
     vx[0] = r.x1 - r.dy * r.width / 2.0; vy[0] = r.y1 + r.dx * r.width / 2.0;
     vx[1] = r.x2 - r.dy * r.width / 2.0; vy[1] = r.y2 + r.dx * r.width / 2.0;
@@ -592,13 +604,13 @@ __device__ __forceinline__ void lsd_rect_count(const LsdFrame& F, const LsdGeom&
             if (y < 0 || y >= F.H) continue;
             ++n;
             const uint32_t wq = __ldg(F.ang + (size_t)y * F.W + x);           // validation runs after k_lsd_regions: the plane is read-only here
-            if (lsd_word_defined(wq) && lsd_aligned_angle(lsd_word_angle(wq), r.theta, r.prec)) ++k;
+            k += lsd_word_aligned(S, wq);
         }
     }
 }
 
 // Point counts of cv2 4.x's rect_nfa enumeration (row spans from lsd_rectenum.h; points outside the image are not counted)
-__device__ __forceinline__ void lsd_rect_count_cv4(const LsdFrame& F, const LsdGeom& g, const LsdRect& r, int& n, int& k) {
+__device__ __forceinline__ void lsd_rect_count_cv4(const LsdFrame& F, const LsdRect& r, const LsdAlignSet& A, int& n, int& k) {
     LsdRowScan S;
     lsd_cv4_setup(r.x1, r.y1, r.x2, r.y2, r.width, r.dx, r.dy, S);
     n = 0; k = 0;
@@ -611,23 +623,24 @@ __device__ __forceinline__ void lsd_rect_count_cv4(const LsdFrame& F, const LsdG
         for (int x = xa; x <= xb; ++x) {
             ++n;
             const uint32_t wq = __ldg(F.ang + (size_t)y * F.W + x);           // validation runs after k_lsd_regions: the plane is read-only here
-            if (lsd_word_defined(wq) && lsd_aligned_angle(lsd_word_angle(wq), r.theta, r.prec)) ++k;
+            k += lsd_word_aligned(A, wq);
         }
     }
 }
 
-__device__ __forceinline__ double lsd_rect_nfa_scalar(const LsdFrame& F, const LsdGeom& g, const LsdRect& r) {
+// rect_nfa of r; S = lsd_align_set(r.theta, r.prec)
+__device__ __forceinline__ double lsd_rect_nfa(const LsdFrame& F, const LsdGeom& g, const LsdRect& r, const LsdAlignSet& S) {
     int n, k;
-    if (g.rect_enum == 1) lsd_rect_count_cv4(F, g, r, n, k);
-    else lsd_rect_count(F, g, r, 0, 1, n, k);
-    return lsd_nfa_scalar(n, k, r.p, g.log_nt, g.lgamma_tab);
+    if (g.rect_enum == 1) lsd_rect_count_cv4(F, r, S, n, k);
+    else lsd_rect_count(F, r, S, 0, 1, n, k);
+    return lsd_nfa(n, k, r.p, g);
 }
 // LineSegmentDetectorImpl::rect_improve after its first NFA evaluation (log_nfa = rect_nfa(rec) <= log_eps), one thread per rectangle.  (A warp per rectangle -
-// lanes sharing the pixel count - was measured 3.8x slower: the NFA itself, log-gamma / pow / log10 in FP64, dominates and is scalar per rectangle, so a warp
-// must carry 32 rectangles to fill its lanes.)
-// Five precisions on one rectangle geometry (the first and the last stage of rect_improve halve p five times without touching the rectangle): the pixel walk and
-// every pixel's angle difference do not depend on the precision, so one pass counts the aligned pixels for all five tolerances.
-__device__ __forceinline__ void lsd_rect_count_cv4_prec5(const LsdFrame& F, const LsdRect& r, const double prec[5], int& n, int k[5]) {
+// lanes sharing the pixel count - was measured 3.8x slower while the NFA was evaluated in FP64 per call; with the NFA a table load and the pixel test integer
+// compares, a lane group per rectangle has not been measured again.)
+// Five precisions on one rectangle geometry (the first and the last stage of rect_improve halve p five times without touching the rectangle): the pixel walk does
+// not depend on the precision, so one pass counts the aligned pixels for all five word sets.
+__device__ __forceinline__ void lsd_rect_count_cv4_prec5(const LsdFrame& F, const LsdRect& r, const LsdAlignSet A[5], int& n, int k[5]) {
     LsdRowScan S;
     lsd_cv4_setup(r.x1, r.y1, r.x2, r.y2, r.width, r.dx, r.dy, S);
     n = 0;
@@ -642,37 +655,36 @@ __device__ __forceinline__ void lsd_rect_count_cv4_prec5(const LsdFrame& F, cons
         for (int x = xa; x <= xb; ++x) {
             ++n;
             const uint32_t wq = __ldg(F.ang + (size_t)y * F.W + x);
-            if (!lsd_word_defined(wq)) continue;
-            double n_theta = r.theta - lsd_word_angle(wq);            // lsd_aligned_angle's difference, compared with each tolerance below
-            if (n_theta < 0) n_theta = -n_theta;
-            if (n_theta > LSD_3_2_PI) { n_theta -= LSD_2PI; if (n_theta < 0) n_theta = -n_theta; }
 #pragma unroll
-            for (int j = 0; j < 5; ++j) k[j] += n_theta <= prec[j];
+            for (int j = 0; j < 5; ++j) k[j] += lsd_word_aligned(A[j], wq);
         }
     }
 }
 __device__ __noinline__ double lsd_rect_improve_rest(const LsdFrame& F, const LsdGeom& g, LsdRect& rec, double log_nfa) {
     const double delta = 0.5, delta_2 = delta / 2.0;
+    LsdAlignSet S;
     for (int stage = 0; stage < 5; ++stage) {
         LsdRect r = rec;
         if ((stage == 0 || stage == 4) && g.rect_enum == 1) {
             if (stage == 0 || (r.width - delta) >= 0.5) {        // (the last stage carries the width test of the stages before it, like OpenCV's)
                 double pv[5], precv[5];
+                LsdAlignSet S5[5];
                 int nn, kk[5];
                 double pp = r.p;
 #pragma unroll
-                for (int n = 0; n < 5; ++n) { pp /= 2; pv[n] = pp; precv[n] = pp * LSD_PI; }
-                lsd_rect_count_cv4_prec5(F, r, precv, nn, kk);
+                for (int n = 0; n < 5; ++n) { pp /= 2; pv[n] = pp; precv[n] = pp * LSD_PI; lsd_align_set(r.theta, precv[n], S5[n]); }
+                lsd_rect_count_cv4_prec5(F, r, S5, nn, kk);
 #pragma unroll
                 for (int n = 0; n < 5; ++n) {
                     r.p = pv[n]; r.prec = precv[n];
-                    const double v = lsd_nfa_scalar(nn, kk[n], r.p, g.log_nt, g.lgamma_tab);
+                    const double v = lsd_nfa(nn, kk[n], r.p, g);
                     if (v > log_nfa) { log_nfa = v; rec = r; }
                 }
             }
             if (stage < 4 && log_nfa > g.log_eps) return log_nfa;
             continue;
         }
+        if (stage == 1) lsd_align_set(rec.theta, rec.prec, S);       // stages 1-3 move and narrow the rectangle but keep its angle and precision
         for (int n = 0; n < 5; ++n) {
             if (stage == 0) { r.p /= 2; r.prec = r.p * LSD_PI; }
             else {
@@ -682,7 +694,8 @@ __device__ __noinline__ double lsd_rect_improve_rest(const LsdFrame& F, const Ls
                 else if (stage == 3) { r.x1 -= -r.dy * delta_2; r.y1 -= r.dx * delta_2; r.x2 -= -r.dy * delta_2; r.y2 -= r.dx * delta_2; r.width -= delta; }
                 else { r.p /= 2; r.prec = r.p * LSD_PI; }
             }
-            const double v = lsd_rect_nfa_scalar(F, g, r);
+            if (stage == 0 || stage == 4) lsd_align_set(r.theta, r.prec, S);
+            const double v = lsd_rect_nfa(F, g, r, S);
             if (v > log_nfa) { log_nfa = v; rec = r; }
         }
         if (stage < 4 && log_nfa > g.log_eps) return log_nfa;
@@ -843,7 +856,9 @@ __global__ void __launch_bounds__(64) k_lsd_validate(LsdGeom g, const uint32_t* 
     F.ang = const_cast<uint32_t*>(ang_all) + (size_t)frame * g.W * g.H; F.cs = nullptr; F.gxy = nullptr; F.reg = nullptr; F.order = nullptr; F.W = g.W; F.H = g.H;
     LsdRect rc;
     lsd_load_cand(cands + ((size_t)frame * g.cand_cap + ci) * 12, rc);
-    const double log_nfa = lsd_rect_nfa_scalar(F, g, rc);
+    LsdAlignSet S;
+    lsd_align_set(rc.theta, rc.prec, S);
+    const double log_nfa = lsd_rect_nfa(F, g, rc, S);
     cand_nfa[(size_t)frame * g.cand_cap + ci] = log_nfa;
     if (!(log_nfa > g.log_eps)) fail_list[(size_t)frame * g.cand_cap + atomicAdd(&n_fail[frame], 1)] = (uint32_t)ci;
 }

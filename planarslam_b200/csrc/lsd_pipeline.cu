@@ -16,7 +16,7 @@ struct LsdBuffers {
     LsdGeom g;
     int max_batch = 0, last_n = 0, max_lines_cap = 0;
     int16_t *d_ix = nullptr, *d_ax = nullptr, *d_iy = nullptr, *d_ay = nullptr;
-    float2* d_lut = nullptr; double* d_lgamma = nullptr;
+    float2* d_lut = nullptr; double* d_lgamma = nullptr; double* d_nfa = nullptr;
     uint8_t* d_gray = nullptr;        // staging for the host-pointer entry points
     uint8_t* d_scaled = nullptr; uint32_t* d_ang = nullptr; float2* d_cs = nullptr; uint32_t* d_gxy = nullptr; int32_t* d_smax = nullptr;
     uint32_t* d_reg = nullptr; uint32_t* d_order = nullptr; int32_t* d_norder = nullptr;
@@ -118,6 +118,7 @@ int lsd_alloc(pslam_ctx* c) {
     const size_t npx = (size_t)g.W * g.H, nb = (size_t)B.max_batch;
 #define LA(ptr, bytes) do { const int rc_ = check_cuda(c, cudaMalloc((void**)&(ptr), (bytes)), "cudaMalloc(lsd)"); if (rc_ != PSLAM_OK) { c->lsd = Bp; lsd_free(c); return rc_; } } while (0)
     LA(B.d_ix, g.W * 2); LA(B.d_ax, g.W * 2); LA(B.d_iy, g.H * 2); LA(B.d_ay, g.H * 2); LA(B.d_lut, lut.size() * sizeof(float2)); LA(B.d_lgamma, LSD_LGAMMA_N * 8);
+    LA(B.d_nfa, (size_t)LSD_NFA_NJ * LSD_NFA_TRI * 8);
     LA(B.d_gray, nb * g.w * g.h); LA(B.d_scaled, nb * npx); LA(B.d_ang, nb * npx * 4); LA(B.d_cs, nb * npx * 8); LA(B.d_gxy, nb * npx * 4); LA(B.d_smax, nb * 4);
     LA(B.d_reg, nb * npx * 4); LA(B.d_order, nb * npx * 4); LA(B.d_norder, nb * 4);
     LA(B.d_fail, nb * g.cand_cap * 4); LA(B.d_nfail, nb * 4);
@@ -132,6 +133,10 @@ int lsd_alloc(pslam_ctx* c) {
     PSLAM_CUDA(c, cudaMemcpyAsync(B.d_lut, lut.data(), lut.size() * sizeof(float2), cudaMemcpyHostToDevice, st));
     PSLAM_CUDA(c, cudaMemcpyAsync(B.d_lgamma, lgam.data(), LSD_LGAMMA_N * 8, cudaMemcpyHostToDevice, st));
     g.lgamma_tab = B.d_lgamma;
+    g.nfa_tab = B.d_nfa;
+    // the NFA table (lsd_nfa): 11 x 131841 entries, evaluated by the device's own lsd_nfa_scalar so that every entry is the double the kernels computed without it
+    k_lsd_nfa_table<<<(LSD_NFA_NJ * LSD_NFA_TRI + 255) / 256, 256, 0, st>>>(g, B.d_nfa);
+    PSLAM_CUDA(c, cudaGetLastError());
     PSLAM_CUDA(c, cudaStreamSynchronize(st));
     c->lsd = Bp;
     return PSLAM_OK;
@@ -140,7 +145,7 @@ int lsd_alloc(pslam_ctx* c) {
 void lsd_free(pslam_ctx* c) {
     if (!c->lsd) return;
     LsdBuffers& B = *c->lsd;
-    for (void* p : {(void*)B.d_ix, (void*)B.d_ax, (void*)B.d_iy, (void*)B.d_ay, (void*)B.d_lut, (void*)B.d_lgamma, (void*)B.d_gray, (void*)B.d_scaled, (void*)B.d_ang, (void*)B.d_cs, (void*)B.d_gxy,
+    for (void* p : {(void*)B.d_ix, (void*)B.d_ax, (void*)B.d_iy, (void*)B.d_ay, (void*)B.d_lut, (void*)B.d_lgamma, (void*)B.d_nfa, (void*)B.d_gray, (void*)B.d_scaled, (void*)B.d_ang, (void*)B.d_cs, (void*)B.d_gxy,
                     (void*)B.d_smax, (void*)B.d_reg, (void*)B.d_order, (void*)B.d_norder, (void*)B.d_segs, (void*)B.d_wpn,
                     (void*)B.d_nsegs, (void*)B.d_status, (void*)B.d_cands, (void*)B.d_cand_nfa, (void*)B.d_ncand, (void*)B.d_fail, (void*)B.d_nfail, (void*)B.d_kl, (void*)B.d_lf, (void*)B.d_nkl, (void*)B.d_dx, (void*)B.d_dy, (void*)B.d_glocal, (void*)B.d_gglobal,
                     (void*)B.d_ldesc, (void*)B.d_lbd72})
