@@ -576,6 +576,23 @@ int pslam_bow_transform(pslam_ctx* ctx, int n_nodes, int L, const uint8_t* voc_d
                         const int32_t* voc_word_id, const double* voc_weight, const uint8_t* features, int n, int levelsup, int32_t* word_id,
                         double* word_val, int32_t* node_id, int32_t* node_off, int32_t* node_feat, int32_t* counts);
 
+/* The vocabulary for the batched transform, uploaded once (ORBvoc.txt is loaded once at System construction, src/System.cc:44) and kept in HBM by
+ * the context: the same flat arrays as pslam_bow_transform in DBoW2's node-id order, child_off[0] = 0, every child id larger than its parent's.
+ * A second call replaces it, n_nodes = 0 releases it.  PSLAM_E_INVALID if a node has more than 32 children.  pslam_bow_transform does not use it. */
+int pslam_bow_set_vocabulary(pslam_ctx* ctx, int n_nodes, int L, const uint8_t* voc_desc, const int32_t* child_off, const int32_t* child_id,
+                             const int32_t* voc_word_id, const double* voc_weight);
+/* Frame::ComputeBoW / KeyFrame::ComputeBoW (transform(desc, mBowVec, mFeatVec, levelsup)) for nframes frames against the resident vocabulary;
+ * PSLAM_E_INVALID if none is set.  desc [nframes][cap][32] with n[f] valid rows (the layout pslam_orb_extract_batch writes), 1 <= cap <= 3072.
+ * Outputs per frame f, each [nframes][cap] (node_off [nframes][cap + 1]): word_id / word_val (BowVector, word ascending), node_id / node_off /
+ * node_feat (FeatureVector CSR, node ascending, features in insertion order); counts [nframes][2] = words, nodes.  Bytes equal pslam_bow_transform's.
+ * The batch size is not bounded by max_batch; device scratch belongs to the context and only grows. */
+int pslam_bow_transform_batch(pslam_ctx* ctx, const uint8_t* desc, const int32_t* n, int cap, int nframes, int levelsup, int32_t* word_id,
+                              double* word_val, int32_t* node_id, int32_t* node_off, int32_t* node_feat, int32_t* counts);
+/* Same with device pointers (d_desc 16-byte aligned; a row count outside [0, cap] is clamped to it); only enqueues on the context's stream
+ * (chains after pslam_orb_extract_batch_dev). */
+int pslam_bow_transform_batch_dev(pslam_ctx* ctx, const uint8_t* d_desc, const int32_t* d_n, int cap, int nframes, int levelsup, int32_t* d_word_id,
+                                  double* d_word_val, int32_t* d_node_id, int32_t* d_node_off, int32_t* d_node_feat, int32_t* d_counts);
+
 /* ---- The RGB-D Frame constructor's compute in one call ----------------------------------------------------
  * Replaces the work of  Frame::Frame(imRGB, imGray, imDepth, ...)   src/Frame.cc:55-140 : the three extractor threads it starts (:90-95)
  *   ExtractORB (:181-186)  then  ComputeStereoFromRGBD (:603-621)            -> mvKeys (= mvKeysUn: no distortion model on this path), mDescriptors, mvuRight, mvDepth

@@ -133,6 +133,9 @@ def lib() -> C.CDLL:
     L.pslam_compute_stereo_from_rgbd_batch.argtypes = [vp, vp, vp, vp, i32, vp, i32, C.c_float, C.c_float, vp, vp]
     L.pslam_compute_stereo_from_rgbd_batch_dev.argtypes = [vp, vp, vp, vp, i32, vp, i32, C.c_float, C.c_float, vp, vp]
     L.pslam_bow_transform.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]
+    L.pslam_bow_set_vocabulary.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp]
+    L.pslam_bow_transform_batch.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+    L.pslam_bow_transform_batch_dev.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]
     L.pslam_search_by_bow.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, vp, i32, vp, vp, i32, vp, vp, vp, C.c_float, i32, vp]
     L.pslam_line_search_by_projection.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, C.c_float, C.c_float, vp]
     _lib = L

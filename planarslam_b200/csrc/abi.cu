@@ -85,6 +85,7 @@ void pslam_destroy(pslam_ctx* c) {
     exchange_free(c);
     planepost_free(c);
     bowdb_free(c);
+    bowvoc_free(c);
     frame_free(c);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     delete c;

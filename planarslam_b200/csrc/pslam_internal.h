@@ -84,6 +84,7 @@ struct TrackBuffers;
 struct ExchangeBuffers;
 struct PlanePostBuffers;
 struct BowDbBuffers;
+struct BowVocBuffers;
 struct FrameBuffers;
 
 }  // namespace pslam
@@ -147,6 +148,7 @@ struct pslam_ctx {
     pslam::PlanePostBuffers* planepost = nullptr; // Frame::ComputePlanes post-processing + surface normals (planepost_kernels.cu)
     pslam::FrameBuffers* frame = nullptr;        // staging of pslam_frame_construct_batch (frame_pipeline.cu)
     pslam::BowDbBuffers* bowdb = nullptr;        // key-frame database BowVectors for loop / relocalisation candidates (bow_kernels.cu)
+    pslam::BowVocBuffers* bowvoc = nullptr;      // resident DBoW2 vocabulary + batched-transform scratch (bow_transform_kernels.cu)
     pslam::ExchangeBuffers* exchange = nullptr;  // key-frame descriptor exchange over peer memory (exchange_kernels.cu)
     // pinned host staging
     uint8_t* h_gray = nullptr; pslam_keypoint* h_kps = nullptr; uint8_t* h_desc = nullptr; int32_t* h_n = nullptr;
@@ -171,6 +173,7 @@ void track_free(pslam_ctx* c);
 void exchange_free(pslam_ctx* c);
 void planepost_free(pslam_ctx* c);
 void bowdb_free(pslam_ctx* c);
+void bowvoc_free(pslam_ctx* c);
 void frame_free(pslam_ctx* c);
 int lsd_status_fetch_async(pslam_ctx* c, int nframes, int32_t* h_pinned);
 // PEAC pipeline (peac_pipeline.cu)

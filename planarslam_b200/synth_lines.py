@@ -93,6 +93,32 @@ def make_vocabulary(seed: int, k: int = 10, L: int = 3, stop_frac: float = 0.05)
                 leaves=np.array(frontier, np.int32))
 
 
+def make_vocabulary_full(seed: int, k: int = 10, L: int = 6, stop_frac: float = 0.05):
+    """A full DBoW2 vocabulary tree of ORBvoc's shape (k = 10, L = 6: 1,111,111 nodes) built level by level with numpy, in the layout of
+    make_vocabulary: level order, the children of a node contiguous, level-1 descriptors random, deeper ones their parent's with about 1/8 of the
+    bits flipped; leaves numbered in level order, weights idf-like with `stop_frac` of them 0."""
+    rng = np.random.Generator(np.random.Philox(key=int(seed) * 37 + 13))
+    sizes = [k ** lv for lv in range(L + 1)]
+    n = sum(sizes)
+    desc = np.zeros((n, 32), np.uint8)
+    desc[1:1 + k] = rng.integers(0, 256, (k, 32), dtype=np.uint8)
+    first = 1                                                   # first node of the current level
+    for lv in range(2, L + 1):
+        parents = np.repeat(np.arange(first, first + sizes[lv - 1]), k)
+        bits = lambda: rng.integers(0, 256, (len(parents), 32), dtype=np.uint8)
+        desc[first + sizes[lv - 1]:first + sizes[lv - 1] + sizes[lv]] = desc[parents] ^ (bits() & bits() & bits())
+        first += sizes[lv - 1]
+    n_inner = n - sizes[L]
+    child_off = np.concatenate([np.arange(n_inner + 1, dtype=np.int64) * k, np.full(sizes[L], n_inner * k)]).astype(np.int32)
+    child_id = np.arange(1, n, dtype=np.int32)
+    leaves = np.arange(n_inner, n, dtype=np.int32)
+    word_id = np.full(n, -1, np.int32)
+    word_id[leaves] = np.arange(sizes[L], dtype=np.int32)
+    weight = np.zeros(n)
+    weight[leaves] = np.where(rng.random(sizes[L]) < stop_frac, 0.0, rng.uniform(0.5, 9.0, sizes[L]))
+    return dict(L=L, k=k, desc=desc, child_off=child_off, child_id=child_id, word_id=word_id, weight=weight, leaves=leaves)
+
+
 def make_features_for_vocabulary(seed: int, voc: dict, n: int = 1000):
     """ORB-like descriptors: noisy copies of random leaf descriptors (so that several features fall into the same word / node)."""
     rng = np.random.Generator(np.random.Philox(key=int(seed) * 77 + 1))
