@@ -59,8 +59,8 @@ int pslam_create(const pslam_config* cfg, pslam_ctx** out) {
     if (rc == PSLAM_OK) rc = peac_build_geometry(c);
     if (rc == PSLAM_OK) rc = check_cuda(c, cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking), "cudaStreamCreate");
     c->stream = c->own_stream;
-    if (rc == PSLAM_OK) rc = check_cuda(c, cudaMalloc((void**)&c->d_status, (size_t)cfg->max_batch * sizeof(int32_t)), "cudaMalloc");
-    if (rc == PSLAM_OK) rc = check_cuda(c, cudaMallocHost((void**)&c->h_status, (size_t)cfg->max_batch * sizeof(int32_t)), "cudaMallocHost");
+    if (rc == PSLAM_OK) rc = c->d_status.reserve(c, cfg->max_batch);
+    if (rc == PSLAM_OK) rc = c->h_status.reserve(c, cfg->max_batch);
     if (rc != PSLAM_OK) {
         std::fprintf(stderr, "pslam_create failed: %s\n", c->err.c_str());
         pslam_destroy(c);
@@ -74,9 +74,6 @@ void pslam_destroy(pslam_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->cfg.device);
     cudaDeviceSynchronize();
-    if (c->orb_ready) orb_free(c);
-    if (c->peac_ready) peac_free(c);
-    cudaFree(c->d_status); cudaFreeHost(c->h_status);
     pose_free(c);
     lba_free(c);
     lsd_free(c);
@@ -88,7 +85,7 @@ void pslam_destroy(pslam_ctx* c) {
     bowvoc_free(c);
     frame_free(c);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
-    delete c;
+    delete c;                                  // frees the ORB / PEAC buffers and the pinned staging
 }
 
 const char* pslam_last_error(const pslam_ctx* c) { return c ? c->err.c_str() : "null context"; }

@@ -110,16 +110,13 @@ __global__ void __launch_bounds__(256) k_bow_orientation(int nf, int32_t* __rest
 
 struct BowDbBuffers {
     int n_kf = 0, total = 0;
-    int32_t* d_off = nullptr; int32_t* d_word = nullptr; double* d_val = nullptr;
-    int32_t* d_common = nullptr; int32_t* d_first = nullptr; float* d_score = nullptr;
-    int32_t* d_qword = nullptr; double* d_qval = nullptr; int q_cap = 0;
+    DevArray<int32_t> d_off, d_word; DevArray<double> d_val;
+    DevArray<int32_t> d_common, d_first; DevArray<float> d_score;
+    DevArray<int32_t> d_qword; DevArray<double> d_qval;
     std::vector<int32_t> h_common, h_first; std::vector<float> h_score;
 };
 
 void bowdb_free(pslam_ctx* c) {
-    if (!c->bowdb) return;
-    BowDbBuffers& B = *c->bowdb;
-    cudaFree(B.d_off); cudaFree(B.d_word); cudaFree(B.d_val); cudaFree(B.d_common); cudaFree(B.d_first); cudaFree(B.d_score); cudaFree(B.d_qword); cudaFree(B.d_qval);
     delete c->bowdb;
     c->bowdb = nullptr;
 }
@@ -183,29 +180,35 @@ int bow_search_impl(pslam_ctx* c, const BowSideArgs& A, const BowSideArgs& Bs, i
     for (int i = 0; i < nffeat; ++i) if (Bs.node_feat[i] < 0 || Bs.node_feat[i] >= nf) return set_error(c, PSLAM_E_INVALID, "frame feature index out of range");
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     cudaStream_t st = c->stream;
-    const size_t sz[] = {pairs.size() * 8, (size_t)nkf * 32, (size_t)nkf * 4, (size_t)nkf, (size_t)(kf_nodes + 1) * 4, (size_t)nkfeat * 4, (size_t)nf * 32,
-                         (size_t)nf * 4, (size_t)(f_nodes + 1) * 4, (size_t)nffeat * 4, (size_t)nf * 4, Bs.has_mp ? (size_t)nf : 0, (size_t)nf, 31 * 4};
-    const void* src[] = {pairs.data(), A.desc, A.angle, A.has_mp, A.node_off, A.node_feat, Bs.desc, Bs.angle, Bs.node_off, Bs.node_feat, match2, Bs.has_mp, nullptr, nullptr};
-    size_t off[15]; off[0] = 0;
-    for (int i = 0; i < 14; ++i) off[i + 1] = (off[i] + sz[i] + 15) & ~(size_t)15;
-    uint8_t* d = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&d, off[14]));
-    cudaError_t e = cudaMemsetAsync(d + off[13], 0, 31 * 4, st);
-    for (int i = 0; i < 12 && e == cudaSuccess; ++i) if (sz[i]) e = cudaMemcpyAsync(d + off[i], src[i], sz[i], cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) { cudaFree(d); return check_cuda(c, e, "SearchByBoW upload"); }
-    int32_t* d_hist = (int32_t*)(d + off[13]);
-    PSLAM_LAUNCH(c, "bow_nodes", k_bow_nodes<<<((int)pairs.size() + 3) / 4, 128, 0, st>>>((int)pairs.size(), (const int2*)(d + off[0]), d + off[1], (const float*)(d + off[2]),
-                 d + off[3], (const int32_t*)(d + off[4]), (const int32_t*)(d + off[5]), d + off[6], (const float*)(d + off[7]), (const int32_t*)(d + off[8]),
-                 (const int32_t*)(d + off[9]), Bs.has_mp ? d + off[11] : nullptr, th_low, nnratio, check_orientation, (int32_t*)(d + off[10]), (int8_t*)(d + off[12]),
-                 d_hist, d_hist + 30));
+    Slab s;
+    const auto d_pairs = s.add<int2>(pairs.size());
+    const auto a_desc = s.add<uint8_t>((size_t)nkf * 32);
+    const auto a_angle = s.add<float>(nkf);
+    const auto a_has_mp = s.add<uint8_t>(nkf);
+    const auto a_node_off = s.add<int32_t>(kf_nodes + 1), a_node_feat = s.add<int32_t>(nkfeat);
+    const auto b_desc = s.add<uint8_t>((size_t)nf * 32);
+    const auto b_angle = s.add<float>(nf);
+    const auto b_node_off = s.add<int32_t>(f_nodes + 1), b_node_feat = s.add<int32_t>(nffeat), d_match = s.add<int32_t>(nf);
+    const auto b_has_mp = s.add<uint8_t>(Bs.has_mp ? nf : 0);
+    const auto d_bin = s.add<int8_t>(nf);
+    const auto d_hist = s.add<int32_t>(30), d_count = s.add<int32_t>(1);     // rotation histogram, number of matches
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    s.zero(d_hist, st); s.zero(d_count, st);
+    s.up(d_pairs, pairs.data(), st); s.up(a_desc, A.desc, st); s.up(a_angle, A.angle, st); s.up(a_has_mp, A.has_mp, st); s.up(a_node_off, A.node_off, st);
+    s.up(a_node_feat, A.node_feat, st); s.up(b_desc, Bs.desc, st); s.up(b_angle, Bs.angle, st); s.up(b_node_off, Bs.node_off, st); s.up(b_node_feat, Bs.node_feat, st);
+    s.up(d_match, match2, st);
+    if (Bs.has_mp) s.up(b_has_mp, Bs.has_mp, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    PSLAM_LAUNCH(c, "bow_nodes", k_bow_nodes<<<((int)pairs.size() + 3) / 4, 128, 0, st>>>((int)pairs.size(), s[d_pairs], s[a_desc], s[a_angle], s[a_has_mp], s[a_node_off],
+                 s[a_node_feat], s[b_desc], s[b_angle], s[b_node_off], s[b_node_feat], Bs.has_mp ? s[b_has_mp] : nullptr, th_low, nnratio, check_orientation, s[d_match],
+                 s[d_bin], s[d_hist], s[d_count]));
     if (check_orientation)
-        PSLAM_LAUNCH(c, "bow_orientation", k_bow_orientation<<<1, 256, 0, st>>>(nf, (int32_t*)(d + off[10]), (const int8_t*)(d + off[12]), d_hist, d_hist + 30));
+        PSLAM_LAUNCH(c, "bow_orientation", k_bow_orientation<<<1, 256, 0, st>>>(nf, s[d_match], s[d_bin], s[d_hist], s[d_count]));
     int32_t n = 0;
-    e = cudaMemcpyAsync(match2, d + off[10], (size_t)nf * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&n, d_hist + 30, 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    if (e != cudaSuccess) return check_cuda(c, e, "SearchByBoW");
+    s.down(match2, d_match, st);
+    s.down(&n, d_count, st);
+    if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
     return n;
 }
 
@@ -217,13 +220,8 @@ int bowdb_score(pslam_ctx* c, int n_q, const int32_t* q_word, const double* q_va
     BowDbBuffers& B = *c->bowdb;
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     cudaStream_t st = c->stream;
-    if (n_q > B.q_cap) {
-        cudaFree(B.d_qword); cudaFree(B.d_qval); B.d_qword = nullptr; B.d_qval = nullptr; B.q_cap = 0;
-        const int cap = std::max(n_q * 3 / 2, 1024);
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_qword, (size_t)cap * 4));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_qval, (size_t)cap * 8));
-        B.q_cap = cap;
-    }
+    int rc;
+    if ((rc = B.d_qword.grow(c, n_q)) || (rc = B.d_qval.grow(c, n_q))) return rc;
     if (n_q) {
         PSLAM_CUDA(c, cudaMemcpyAsync(B.d_qword, q_word, (size_t)n_q * 4, cudaMemcpyHostToDevice, st));
         PSLAM_CUDA(c, cudaMemcpyAsync(B.d_qval, q_val, (size_t)n_q * 8, cudaMemcpyHostToDevice, st));
@@ -285,13 +283,13 @@ extern "C" int pslam_bow_database_set(pslam_ctx* c, int n_kf, const int32_t* kf_
     c->bowdb = new BowDbBuffers();
     BowDbBuffers& B = *c->bowdb;
     B.n_kf = n_kf; B.total = total;
-    cudaError_t e = cudaMalloc((void**)&B.d_off, (size_t)(n_kf + 1) * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&B.d_word, (size_t)std::max(total, 1) * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&B.d_val, (size_t)std::max(total, 1) * 8);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&B.d_common, (size_t)n_kf * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&B.d_first, (size_t)n_kf * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&B.d_score, (size_t)n_kf * 4);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(B.d_off, kf_off, (size_t)(n_kf + 1) * 4, cudaMemcpyHostToDevice, c->stream);
+    int rc;
+    if ((rc = B.d_off.reserve(c, n_kf + 1)) || (rc = B.d_word.reserve(c, total)) || (rc = B.d_val.reserve(c, total)) || (rc = B.d_common.reserve(c, n_kf)) ||
+        (rc = B.d_first.reserve(c, n_kf)) || (rc = B.d_score.reserve(c, n_kf))) {
+        bowdb_free(c);
+        return rc;
+    }
+    cudaError_t e = cudaMemcpyAsync(B.d_off, kf_off, (size_t)(n_kf + 1) * 4, cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess && total) e = cudaMemcpyAsync(B.d_word, kf_word, (size_t)total * 4, cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess && total) e = cudaMemcpyAsync(B.d_val, kf_val, (size_t)total * 8, cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);

@@ -113,24 +113,20 @@ __global__ void __launch_bounds__(256) k_bow_assemble(int n, const int32_t* __re
 // The vocabulary kept in HBM, in child-slot order (slot c = position c of the flat child_id array): the children of a node are adjacent
 struct BowVocBuffers {
     int n_nodes = 0, L = 0, max_k = 0, root_c0 = 0, root_nc = 0;
-    uint8_t* d_cdesc = nullptr;     // [n_child][32] descriptor of the node in slot c
-    int4* d_cinfo = nullptr;        // {first child slot, number of children, node id, word id} of the node in slot c
-    double* d_cweight = nullptr;    // weight of the node in slot c
+    DevArray<uint8_t> d_cdesc;      // [n_child][32] descriptor of the node in slot c
+    DevArray<int4> d_cinfo;         // {first child slot, number of children, node id, word id} of the node in slot c
+    DevArray<double> d_cweight;     // weight of the node in slot c
     // scratch of the batch calls (only grows)
-    uint8_t* d_feat = nullptr; size_t feat_bytes = 0;      // per feature: word, node, weight
-    uint8_t* d_stage = nullptr; size_t stage_bytes = 0;    // host-pointer entry point: inputs and outputs
+    DevArray<uint8_t> d_feat;       // per feature: word, node, weight
+    DevArray<uint8_t> d_stage;      // host-pointer entry point: inputs and outputs
 };
 
 static void bowvoc_release_vocabulary(BowVocBuffers& V) {
-    cudaFree(V.d_cdesc); cudaFree(V.d_cinfo); cudaFree(V.d_cweight);
-    V.d_cdesc = nullptr; V.d_cinfo = nullptr; V.d_cweight = nullptr;
+    V.d_cdesc.release(); V.d_cinfo.release(); V.d_cweight.release();
     V.n_nodes = V.L = V.max_k = V.root_c0 = V.root_nc = 0;
 }
 
 void bowvoc_free(pslam_ctx* c) {
-    if (!c->bowvoc) return;
-    bowvoc_release_vocabulary(*c->bowvoc);
-    cudaFree(c->bowvoc->d_feat); cudaFree(c->bowvoc->d_stage);
     delete c->bowvoc;
     c->bowvoc = nullptr;
 }
@@ -281,14 +277,6 @@ __global__ void __launch_bounds__(BOW_ASM_THREADS) k_bow_assemble_batch(int cap,
 
 namespace {
 
-int grow(pslam_ctx* c, uint8_t** p, size_t* have, size_t need) {
-    if (need <= *have) return PSLAM_OK;
-    cudaFree(*p); *p = nullptr; *have = 0;
-    PSLAM_CUDA(c, cudaMalloc((void**)p, need));
-    *have = need;
-    return PSLAM_OK;
-}
-
 int bow_batch_check(pslam_ctx* c, int cap, int nframes) {
     if (!c->bowvoc || !c->bowvoc->n_nodes) return set_error(c, PSLAM_E_INVALID, "no resident vocabulary (pslam_bow_set_vocabulary)");
     if (nframes < 0 || cap < 1 || cap > BOW_MAX_FEATURES) return set_error(c, PSLAM_E_INVALID, "bad batch shape (1 <= cap <= 3072 features per frame)");
@@ -301,9 +289,9 @@ int bow_batch_run(pslam_ctx* c, const uint8_t* d_desc, const int32_t* d_n, int c
                   int32_t* d_node_id, int32_t* d_node_off, int32_t* d_node_feat, int32_t* d_counts) {
     BowVocBuffers& V = *c->bowvoc;
     const long long total = (long long)nframes * cap;
-    int rc = grow(c, &V.d_feat, &V.feat_bytes, (size_t)total * 16);
+    const int rc = V.d_feat.reserve(c, (size_t)total * 16);
     if (rc != PSLAM_OK) return rc;
-    int32_t* f_word = (int32_t*)V.d_feat;
+    int32_t* f_word = reinterpret_cast<int32_t*>(V.d_feat.ptr);
     int32_t* f_node = f_word + total;
     double* f_weight = (double*)(f_node + total);
     cudaStream_t st = c->stream;
@@ -340,33 +328,33 @@ extern "C" int pslam_bow_transform(pslam_ctx* c, int n_nodes, int L, const uint8
     cudaStream_t st = c->stream;
     const int n_child = child_off[n_nodes];
     // a caller that transforms many frames keeps the vocabulary resident; this entry point uploads it per call for simplicity
-    const size_t sz[] = {(size_t)n_nodes * 32, (size_t)(n_nodes + 1) * 4, (size_t)n_child * 4, (size_t)n_nodes * 4, (size_t)n_nodes * 8, (size_t)n * 32,
-                         (size_t)n * 4, (size_t)n * 4, (size_t)n * 8, (size_t)n * 4, (size_t)n * 8, (size_t)n * 4, (size_t)(n + 1) * 4, (size_t)n * 4, 8};
-    const void* src[] = {voc_desc, child_off, child_id, voc_word_id, voc_weight, features};
-    size_t off[16]; off[0] = 0;
-    for (int i = 0; i < 15; ++i) off[i + 1] = (off[i] + sz[i] + 15) & ~(size_t)15;
-    uint8_t* d = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&d, off[15]));
-    cudaError_t e = cudaSuccess;
-    for (int i = 0; i < 6 && e == cudaSuccess; ++i) e = cudaMemcpyAsync(d + off[i], src[i], sz[i], cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) { cudaFree(d); return check_cuda(c, e, "bow transform upload"); }
-    PSLAM_LAUNCH(c, "bow_descend", k_bow_descend<<<(n + 3) / 4, 128, 0, st>>>(n, L, levelsup, d + off[0], (const int32_t*)(d + off[1]), (const int32_t*)(d + off[2]),
-                 (const int32_t*)(d + off[3]), (const double*)(d + off[4]), d + off[5], (int32_t*)(d + off[6]), (int32_t*)(d + off[7]), (double*)(d + off[8])));
-    PSLAM_LAUNCH(c, "bow_assemble", k_bow_assemble<<<1, 256, 0, st>>>(n, (const int32_t*)(d + off[6]), (const int32_t*)(d + off[7]), (const double*)(d + off[8]),
-                 (int32_t*)(d + off[9]), (double*)(d + off[10]), (int32_t*)(d + off[11]), (int32_t*)(d + off[12]), (int32_t*)(d + off[13]), (int32_t*)(d + off[14])));
+    Slab s;
+    const auto v_desc = s.add<uint8_t>((size_t)n_nodes * 32);
+    const auto v_child_off = s.add<int32_t>(n_nodes + 1), v_child_id = s.add<int32_t>(n_child), v_word_id = s.add<int32_t>(n_nodes);
+    const auto v_weight = s.add<double>(n_nodes);
+    const auto feat = s.add<uint8_t>((size_t)n * 32);
+    const auto f_word = s.add<int32_t>(n), f_node = s.add<int32_t>(n);
+    const auto f_weight = s.add<double>(n);
+    const auto d_word_id = s.add<int32_t>(n);
+    const auto d_word_val = s.add<double>(n);
+    const auto d_node_id = s.add<int32_t>(n), d_node_off = s.add<int32_t>(n + 1), d_node_feat = s.add<int32_t>(n), d_counts = s.add<int32_t>(2);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    s.up(v_desc, voc_desc, st); s.up(v_child_off, child_off, st); s.up(v_child_id, child_id, st); s.up(v_word_id, voc_word_id, st); s.up(v_weight, voc_weight, st);
+    s.up(feat, features, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    PSLAM_LAUNCH(c, "bow_descend", k_bow_descend<<<(n + 3) / 4, 128, 0, st>>>(n, L, levelsup, s[v_desc], s[v_child_off], s[v_child_id], s[v_word_id], s[v_weight], s[feat],
+                 s[f_word], s[f_node], s[f_weight]));
+    PSLAM_LAUNCH(c, "bow_assemble", k_bow_assemble<<<1, 256, 0, st>>>(n, s[f_word], s[f_node], s[f_weight], s[d_word_id], s[d_word_val], s[d_node_id], s[d_node_off],
+                 s[d_node_feat], s[d_counts]));
     int32_t cnt[2] = {0, 0};
-    e = cudaMemcpyAsync(cnt, d + off[14], 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess && cnt[0] > 0) {
-        e = cudaMemcpyAsync(word_id, d + off[9], (size_t)cnt[0] * 4, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(word_val, d + off[10], (size_t)cnt[0] * 8, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(node_id, d + off[11], (size_t)cnt[1] * 4, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(node_off, d + off[12], (size_t)(cnt[1] + 1) * 4, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(node_feat, d + off[13], (size_t)n * 4, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    s.down(cnt, d_counts, st);
+    if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
+    if (cnt[0] > 0) {
+        s.down(word_id, d_word_id, st, cnt[0]); s.down(word_val, d_word_val, st, cnt[0]); s.down(node_id, d_node_id, st, cnt[1]);
+        s.down(node_off, d_node_off, st, cnt[1] + 1); s.down(node_feat, d_node_feat, st);
+        if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
     }
-    cudaFree(d);
-    if (e != cudaSuccess) return check_cuda(c, e, "bow transform");
     counts[0] = cnt[0]; counts[1] = cnt[1];
     return PSLAM_OK;
 }
@@ -402,10 +390,12 @@ extern "C" int pslam_bow_set_vocabulary(pslam_ctx* c, int n_nodes, int L, const 
     if (!c->bowvoc) c->bowvoc = new BowVocBuffers();
     BowVocBuffers& V = *c->bowvoc;
     bowvoc_release_vocabulary(V);
-    cudaError_t e = cudaMalloc((void**)&V.d_cdesc, cdesc.size());
-    if (e == cudaSuccess) e = cudaMalloc((void**)&V.d_cinfo, cinfo.size() * sizeof(int4));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&V.d_cweight, cweight.size() * 8);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(V.d_cdesc, cdesc.data(), cdesc.size(), cudaMemcpyHostToDevice, c->stream);
+    int rc;
+    if ((rc = V.d_cdesc.reserve(c, cdesc.size())) || (rc = V.d_cinfo.reserve(c, cinfo.size())) || (rc = V.d_cweight.reserve(c, cweight.size()))) {
+        bowvoc_release_vocabulary(V);
+        return rc;
+    }
+    cudaError_t e = cudaMemcpyAsync(V.d_cdesc, cdesc.data(), cdesc.size(), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(V.d_cinfo, cinfo.data(), cinfo.size() * sizeof(int4), cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(V.d_cweight, cweight.data(), cweight.size() * 8, cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
@@ -437,22 +427,19 @@ extern "C" int pslam_bow_transform_batch(pslam_ctx* c, const uint8_t* desc, cons
         if (n[f] < 0 || n[f] > cap) return set_error(c, PSLAM_E_INVALID, "n[f] must lie in [0, cap] (at most 3072 features per frame)");
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     const size_t nf = (size_t)nframes * cap;
-    // staging: desc, n, word_id, word_val, node_id, node_off, node_feat, counts
-    const size_t sz[] = {nf * 32, (size_t)nframes * 4, nf * 4, nf * 8, nf * 4, (size_t)nframes * (cap + 1) * 4, nf * 4, (size_t)nframes * 8};
-    size_t off[9]; off[0] = 0;
-    for (int i = 0; i < 8; ++i) off[i + 1] = (off[i] + sz[i] + 255) & ~(size_t)255;
-    BowVocBuffers& V = *c->bowvoc;
-    rc = grow(c, &V.d_stage, &V.stage_bytes, off[8]);
-    if (rc != PSLAM_OK) return rc;
-    uint8_t* d = V.d_stage;
+    Slab s;
+    const auto d_desc = s.add<uint8_t>(nf * 32);
+    const auto d_n = s.add<int32_t>(nframes), d_word_id = s.add<int32_t>(nf);
+    const auto d_word_val = s.add<double>(nf);
+    const auto d_node_id = s.add<int32_t>(nf), d_node_off = s.add<int32_t>((size_t)nframes * (cap + 1)), d_node_feat = s.add<int32_t>(nf);
+    const auto d_counts = s.add<int32_t>((size_t)nframes * 2);
+    if ((rc = s.alloc(c, c->bowvoc->d_stage)) != PSLAM_OK) return rc;
     cudaStream_t st = c->stream;
-    PSLAM_CUDA(c, cudaMemcpyAsync(d + off[0], desc, sz[0], cudaMemcpyHostToDevice, st));
-    PSLAM_CUDA(c, cudaMemcpyAsync(d + off[1], n, sz[1], cudaMemcpyHostToDevice, st));
-    rc = bow_batch_run(c, d + off[0], (const int32_t*)(d + off[1]), cap, nframes, levelsup, (int32_t*)(d + off[2]), (double*)(d + off[3]), (int32_t*)(d + off[4]),
-                       (int32_t*)(d + off[5]), (int32_t*)(d + off[6]), (int32_t*)(d + off[7]));
+    s.up(d_desc, desc, st); s.up(d_n, n, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    rc = bow_batch_run(c, s[d_desc], s[d_n], cap, nframes, levelsup, s[d_word_id], s[d_word_val], s[d_node_id], s[d_node_off], s[d_node_feat], s[d_counts]);
     if (rc != PSLAM_OK) return rc;
-    void* dst[] = {word_id, word_val, node_id, node_off, node_feat, counts};
-    for (int i = 0; i < 6; ++i) PSLAM_CUDA(c, cudaMemcpyAsync(dst[i], d + off[i + 2], sz[i + 2], cudaMemcpyDeviceToHost, st));
-    PSLAM_CUDA(c, cudaStreamSynchronize(st));
-    return PSLAM_OK;
+    s.down(word_id, d_word_id, st); s.down(word_val, d_word_val, st); s.down(node_id, d_node_id, st); s.down(node_off, d_node_off, st);
+    s.down(node_feat, d_node_feat, st); s.down(counts, d_counts, st);
+    return s.sync(c, st);
 }

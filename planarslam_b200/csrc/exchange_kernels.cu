@@ -28,12 +28,12 @@ namespace pslam {
 struct ExchangeBuffers {
     int cap = 0, slots = 0, world = 1, rank = 0;
     size_t slot_bytes = 0;
-    uint8_t* local = nullptr;                       // this rank's block
+    DevArray<uint8_t> local;                        // this rank's block
     uint8_t* peer[XCH_MAX_WORLD] = {nullptr};       // mapped blocks (peer[rank] == local)
     bool opened[XCH_MAX_WORLD] = {false};
-    uint32_t* d_part = nullptr;                     // [XCH_MAX_WORLD][capq][2] per-peer best keys
-    int32_t* d_ticket = nullptr;                    // per query tile
-    int32_t* d_timeouts = nullptr;                  // CTAs that gave up waiting for a peer's epoch flag (pslam_exchange_timeouts)
+    DevArray<uint32_t> d_part;                      // [XCH_MAX_WORLD][capq][2] per-peer best keys
+    DevArray<int32_t> d_ticket;                     // per query tile
+    DevArray<int32_t> d_timeouts;                   // CTAs that gave up waiting for a peer's epoch flag (pslam_exchange_timeouts)
     int capq = 0;
 };
 
@@ -177,8 +177,7 @@ __global__ void __launch_bounds__(XCH_WARPS * 32) k_exchange_match(ExchangePeers
 void exchange_free(pslam_ctx* c) {
     if (!c->exchange) return;
     ExchangeBuffers& B = *c->exchange;
-    for (int r = 0; r < B.world; ++r) if (B.opened[r] && B.peer[r]) cudaIpcCloseMemHandle(B.peer[r]);
-    cudaFree(B.local); cudaFree(B.d_part); cudaFree(B.d_ticket); cudaFree(B.d_timeouts);
+    for (int r = 0; r < B.world; ++r) if (B.opened[r] && B.peer[r]) cudaIpcCloseMemHandle(B.peer[r]);      // before the local block goes
     delete c->exchange;
     c->exchange = nullptr;
 }
@@ -197,9 +196,10 @@ int pslam_exchange_create(pslam_ctx* c, int cap_kp, int slots, void* ipc_handle_
     c->exchange = new ExchangeBuffers();
     ExchangeBuffers& B = *c->exchange;
     B.cap = cap_kp; B.slots = slots; B.slot_bytes = xch_slot_bytes(cap_kp);
-    PSLAM_CUDA(c, cudaMalloc((void**)&B.local, B.slot_bytes * slots));
+    int rc;
+    if ((rc = B.local.reserve(c, B.slot_bytes * slots))) return rc;
     PSLAM_CUDA(c, cudaMemset(B.local, 0, B.slot_bytes * slots));
-    PSLAM_CUDA(c, cudaMalloc((void**)&B.d_timeouts, 4));
+    if ((rc = B.d_timeouts.reserve(c, 1))) return rc;
     PSLAM_CUDA(c, cudaMemset(B.d_timeouts, 0, 4));
     B.peer[0] = B.local; B.world = 1; B.rank = 0;
     cudaIpcMemHandle_t h;
@@ -246,9 +246,8 @@ int pslam_exchange_match_dev(pslam_ctx* c, int slot, uint32_t epoch, const uint8
     ExchangeBuffers& B = *c->exchange;
     const int tiles = (capq + XCH_WARPS * XCH_NQ - 1) / (XCH_WARPS * XCH_NQ);
     if (capq > B.capq) {
-        cudaFree(B.d_part); cudaFree(B.d_ticket); B.d_part = nullptr; B.d_ticket = nullptr; B.capq = 0;
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_part, (size_t)XCH_MAX_WORLD * capq * 2 * 4));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_ticket, (size_t)tiles * 4));
+        int rc;
+        if ((rc = B.d_part.reserve(c, (size_t)XCH_MAX_WORLD * capq * 2)) || (rc = B.d_ticket.reserve(c, tiles))) return rc;
         PSLAM_CUDA(c, cudaMemsetAsync(B.d_ticket, 0, (size_t)tiles * 4, c->stream));
         B.capq = capq;
     }

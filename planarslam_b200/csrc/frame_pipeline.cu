@@ -16,18 +16,14 @@
 namespace pslam {
 
 struct FrameBuffers {
-    size_t cap_bytes = 0;
-    uint8_t* d = nullptr;          // one slab, carved up per call
-    int32_t* h_status = nullptr;   // pinned
-    int h_status_cap = 0;
+    DevArray<uint8_t> slab;        // carved up per call
+    PinnedArray<int32_t> h_status;
     cudaStream_t copy = nullptr;   // second stream: gray upload / plane-product download next to the kernels
     cudaEvent_t ev_gray = nullptr, ev_planes = nullptr, ev_idle = nullptr;
 };
 
 void frame_free(pslam_ctx* c) {
     if (!c->frame) return;
-    cudaFree(c->frame->d);
-    if (c->frame->h_status) cudaFreeHost(c->frame->h_status);
     if (c->frame->copy) cudaStreamDestroy(c->frame->copy);
     for (cudaEvent_t e : {c->frame->ev_gray, c->frame->ev_planes, c->frame->ev_idle}) if (e) cudaEventDestroy(e);
     delete c->frame;
@@ -52,81 +48,80 @@ int pslam_frame_construct_batch(pslam_ctx* c, const uint8_t* gray, const uint16_
     if (!c->frame) c->frame = new FrameBuffers();
     FrameBuffers& B = *c->frame;
     const size_t npx = (size_t)c->cfg.width * c->cfg.height, nf = (size_t)nframes, ml = (size_t)max_lines, cp = (size_t)out->cap_plane_pts;
-    enum { GRAY, DEPTH, KPS, DESC, NK, UR, DZ, KL, LF, LDESC, L3D, NKL, SEED, DRAWN, LABELS, PLANES, NPL, MEMBERS, MOFF, PPN, PPSRC, PPCOEF, PPOFF, PPPTS, PPST, SN8, NSEG };
-    const size_t sz[NSEG] = {nf * npx, nf * npx * 2, nf * cap * sizeof(pslam_keypoint), nf * cap * 32, nf * 4, nf * cap * 4, nf * cap * 4,
-                             nf * ml * sizeof(pslam_keyline), nf * ml * 24, nf * ml * 32, nf * ml * sizeof(pslam_line3d), nf * 4, nf * 4, nf * 4,
-                             nf * npx * 4, nf * maxp * sizeof(pslam_plane), nf * 4, nf * npx * 4, nf * (maxp + 1) * 4,
-                             nf * 4, nf * maxp * 4, nf * maxp * 16, nf * (maxp + 1) * 4, nf * cp * 12, nf * 4, out->surface_normals8 ? nf * n_sn * 32 : 0};
-    size_t off[NSEG + 1];
-    off[0] = 0;
-    for (int i = 0; i < NSEG; ++i) off[i + 1] = (off[i] + sz[i] + 255) & ~(size_t)255;
-    if (off[NSEG] > B.cap_bytes) {
-        PSLAM_CUDA(c, cudaStreamSynchronize(c->stream));
-        cudaFree(B.d); B.d = nullptr; B.cap_bytes = 0;
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d, off[NSEG]));
-        B.cap_bytes = off[NSEG];
-    }
-    if (nframes > B.h_status_cap) {
-        if (B.h_status) cudaFreeHost(B.h_status);
-        B.h_status = nullptr; B.h_status_cap = 0;
-        PSLAM_CUDA(c, cudaMallocHost((void**)&B.h_status, (size_t)nframes * 4 * sizeof(int32_t)));
-        B.h_status_cap = nframes;
-    }
+    Slab s;
+    const auto gray_d = s.add<uint8_t>(nf * npx);
+    const auto depth_d = s.add<uint16_t>(nf * npx);
+    const auto kps = s.add<pslam_keypoint>(nf * cap);
+    const auto desc = s.add<uint8_t>(nf * cap * 32);
+    const auto nk = s.add<int32_t>(nf);
+    const auto ur = s.add<float>(nf * cap), dz = s.add<float>(nf * cap);
+    const auto kl = s.add<pslam_keyline>(nf * ml);
+    const auto lf = s.add<double>(nf * ml * 3);
+    const auto ldesc = s.add<uint8_t>(nf * ml * 32);
+    const auto l3d = s.add<pslam_line3d>(nf * ml);
+    const auto nkl = s.add<int32_t>(nf);
+    const auto seed = s.add<uint32_t>(nf);
+    const auto drawn = s.add<int32_t>(nf), labels = s.add<int32_t>(nf * npx);
+    const auto planes = s.add<pslam_plane>(nf * maxp);
+    const auto npl = s.add<int32_t>(nf), members = s.add<int32_t>(nf * npx), moff = s.add<int32_t>(nf * (maxp + 1)), ppn = s.add<int32_t>(nf), ppsrc = s.add<int32_t>(nf * maxp);
+    const auto ppcoef = s.add<float>(nf * maxp * 4);
+    const auto ppoff = s.add<int32_t>(nf * (maxp + 1));
+    const auto pppts = s.add<float>(nf * cp * 3);
+    const auto ppst = s.add<int32_t>(nf);
+    const auto sn8 = s.add<float>(out->surface_normals8 ? nf * n_sn * 8 : 0);
+    int rc;
+    if (s.bytes() > B.slab.cap) PSLAM_CUDA(c, cudaStreamSynchronize(c->stream));      // an earlier call's kernels may still read the old slab
+    if ((rc = s.alloc(c, B.slab)) || (rc = B.h_status.reserve(c, nf * 4))) return rc;
     if (!B.copy) {
         PSLAM_CUDA(c, cudaStreamCreateWithFlags(&B.copy, cudaStreamNonBlocking));
         PSLAM_CUDA(c, cudaEventCreateWithFlags(&B.ev_gray, cudaEventDisableTiming));
         PSLAM_CUDA(c, cudaEventCreateWithFlags(&B.ev_planes, cudaEventDisableTiming));
         PSLAM_CUDA(c, cudaEventCreateWithFlags(&B.ev_idle, cudaEventDisableTiming));
     }
-    uint8_t* d = B.d;
-#define SEG(T, i) reinterpret_cast<T*>(d + off[i])
-#define BACK(stream, dst, i) PSLAM_CUDA(c, cudaMemcpyAsync((dst), d + off[i], sz[i], cudaMemcpyDeviceToHost, (stream)))
     cudaStream_t st = c->stream, cs = B.copy;
     // the copy stream starts after whatever the context's stream still holds (an earlier call's kernels may read the slab)
     PSLAM_CUDA(c, cudaEventRecord(B.ev_idle, st));
     PSLAM_CUDA(c, cudaStreamWaitEvent(cs, B.ev_idle, 0));
-    PSLAM_CUDA(c, cudaMemcpyAsync(SEG(uint16_t, DEPTH), depth, sz[DEPTH], cudaMemcpyHostToDevice, st));
-    PSLAM_CUDA(c, cudaMemcpyAsync(SEG(uint8_t, GRAY), gray, sz[GRAY], cudaMemcpyHostToDevice, cs));
+    s.up(depth_d, depth, st);
+    s.up(gray_d, gray, cs);
     PSLAM_CUDA(c, cudaEventRecord(B.ev_gray, cs));
     {   // one rand() stream per frame, all started from the caller's seed (pslam_lines3d_batch documents the single-stream alternative)
         for (int f = 0; f < nframes; ++f) B.h_status[f] = (int32_t)line_seed;
-        PSLAM_CUDA(c, cudaMemcpyAsync(SEG(uint32_t, SEED), B.h_status, nf * 4, cudaMemcpyHostToDevice, st));
+        s.up(seed, reinterpret_cast<const uint32_t*>(B.h_status.ptr), st);
     }
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
     const float cam[4] = {c->cfg.fx, c->cfg.fy, c->cfg.cx, c->cfg.cy};
-    int rc;
     // ComputePlanes on the depth frames while the gray frames arrive
-    if ((rc = pslam_peac_run_batch_dev(c, SEG(uint16_t, DEPTH), nframes, SEG(int32_t, LABELS), SEG(pslam_plane, PLANES), SEG(int32_t, NPL), SEG(int32_t, MEMBERS), SEG(int32_t, MOFF))) != PSLAM_OK)
+    if ((rc = pslam_peac_run_batch_dev(c, s[depth_d], nframes, s[labels], s[planes], s[npl], s[members], s[moff])) != PSLAM_OK)
         return rc;
-    if ((rc = pslam_planes_post_batch_dev(c, SEG(uint16_t, DEPTH), nframes, SEG(pslam_plane, PLANES), SEG(int32_t, NPL), SEG(int32_t, MEMBERS), SEG(int32_t, MOFF), plane_dist_th,
-                                          SEG(int32_t, PPN), SEG(int32_t, PPSRC), SEG(float, PPCOEF), SEG(int32_t, PPOFF), SEG(float, PPPTS), out->cap_plane_pts, SEG(int32_t, PPST))) != PSLAM_OK)
+    if ((rc = pslam_planes_post_batch_dev(c, s[depth_d], nframes, s[planes], s[npl], s[members], s[moff], plane_dist_th,
+                                          s[ppn], s[ppsrc], s[ppcoef], s[ppoff], s[pppts], out->cap_plane_pts, s[ppst])) != PSLAM_OK)
         return rc;
-    if (out->surface_normals8 && (rc = pslam_surface_normals_batch_dev(c, SEG(uint16_t, DEPTH), nframes, SEG(float, SN8), nullptr)) != PSLAM_OK) return rc;
+    if (out->surface_normals8 && (rc = pslam_surface_normals_batch_dev(c, s[depth_d], nframes, s[sn8], nullptr)) != PSLAM_OK) return rc;
     PSLAM_CUDA(c, cudaMemcpyAsync(B.h_status + 2 * (size_t)nframes, c->d_status, nf * 4, cudaMemcpyDeviceToHost, st));      // PEAC capacity flags (ORB reuses the array below)
     PSLAM_CUDA(c, cudaEventRecord(B.ev_planes, st));
     // the plane products return on the copy stream while the two image chains run
     PSLAM_CUDA(c, cudaStreamWaitEvent(cs, B.ev_planes, 0));
-    BACK(cs, out->n_planes, PPN); BACK(cs, out->plane_src, PPSRC); BACK(cs, out->plane_coef, PPCOEF); BACK(cs, out->plane_pt_off, PPOFF); BACK(cs, out->plane_pts, PPPTS);
-    if (out->surface_normals8) BACK(cs, out->surface_normals8, SN8);
-    PSLAM_CUDA(c, cudaMemcpyAsync(B.h_status + (size_t)nframes, d + off[PPST], nf * 4, cudaMemcpyDeviceToHost, cs));        // plane post-processing capacity flags
+    s.down(out->n_planes, ppn, cs); s.down(out->plane_src, ppsrc, cs); s.down(out->plane_coef, ppcoef, cs); s.down(out->plane_pt_off, ppoff, cs); s.down(out->plane_pts, pppts, cs);
+    if (out->surface_normals8) s.down(out->surface_normals8, sn8, cs);
+    s.down(B.h_status + nframes, ppst, cs);        // plane post-processing capacity flags
     // ExtractORB, then ComputeStereoFromRGBD on the key points it leaves in HBM (no distortion model on this path: mvKeysUn = mvKeys, Frame::UndistortKeyPoints :545-549)
     PSLAM_CUDA(c, cudaStreamWaitEvent(st, B.ev_gray, 0));
-    if ((rc = pslam_orb_extract_batch_dev(c, SEG(uint8_t, GRAY), nframes, SEG(pslam_keypoint, KPS), SEG(uint8_t, DESC), cap, SEG(int32_t, NK))) != PSLAM_OK) return rc;
-    if ((rc = pslam_compute_stereo_from_rgbd_batch_dev(c, SEG(pslam_keypoint, KPS), SEG(pslam_keypoint, KPS), SEG(int32_t, NK), cap, SEG(uint16_t, DEPTH), nframes, depth_factor, bf,
-                                                       SEG(float, UR), SEG(float, DZ))) != PSLAM_OK) return rc;
+    if ((rc = pslam_orb_extract_batch_dev(c, s[gray_d], nframes, s[kps], s[desc], cap, s[nk])) != PSLAM_OK) return rc;
+    if ((rc = pslam_compute_stereo_from_rgbd_batch_dev(c, s[kps], s[kps], s[nk], cap, s[depth_d], nframes, depth_factor, bf,
+                                                       s[ur], s[dz])) != PSLAM_OK) return rc;
     PSLAM_CUDA(c, cudaMemcpyAsync(B.h_status, c->d_status, nf * 4, cudaMemcpyDeviceToHost, st));                            // ORB capacity flags
-    BACK(st, out->keys, KPS); BACK(st, out->desc, DESC); BACK(st, out->n_keys, NK); BACK(st, out->u_right, UR); BACK(st, out->depth_kp, DZ);
+    s.down(out->keys, kps, st); s.down(out->desc, desc, st); s.down(out->n_keys, nk, st); s.down(out->u_right, ur, st); s.down(out->depth_kp, dz, st);
     // ExtractLSD: segments -> key lines + line functions + LBD descriptors, then isLineGood
-    if ((rc = pslam_lines_extract_describe_batch_dev(c, SEG(uint8_t, GRAY), nframes, max_lines, SEG(pslam_keyline, KL), SEG(double, LF), SEG(uint8_t, LDESC), SEG(int32_t, NKL))) != PSLAM_OK)
+    if ((rc = pslam_lines_extract_describe_batch_dev(c, s[gray_d], nframes, max_lines, s[kl], s[lf], s[ldesc], s[nkl])) != PSLAM_OK)
         return rc;
-    if ((rc = pslam_lines3d_batch_dev(c, SEG(pslam_keyline, KL), SEG(int32_t, NKL), max_lines, SEG(uint16_t, DEPTH), nframes, depth_factor, cam, SEG(uint32_t, SEED), nullptr,
-                                      SEG(pslam_line3d, L3D), SEG(int32_t, DRAWN))) != PSLAM_OK) return rc;
+    if ((rc = pslam_lines3d_batch_dev(c, s[kl], s[nkl], max_lines, s[depth_d], nframes, depth_factor, cam, s[seed], nullptr,
+                                      s[l3d], s[drawn])) != PSLAM_OK) return rc;
     if ((rc = lsd_status_fetch_async(c, nframes, B.h_status + 3 * (size_t)nframes)) != PSLAM_OK) return rc;
-    BACK(st, out->keylines, KL); BACK(st, out->line_functions, LF); BACK(st, out->line_desc, LDESC); BACK(st, out->lines3d, L3D); BACK(st, out->n_lines, NKL);
-    if (out->n_rand_drawn) BACK(st, out->n_rand_drawn, DRAWN);
-#undef BACK
-#undef SEG
+    s.down(out->keylines, kl, st); s.down(out->line_functions, lf, st); s.down(out->line_desc, ldesc, st); s.down(out->lines3d, l3d, st); s.down(out->n_lines, nkl, st);
+    if (out->n_rand_drawn) s.down(out->n_rand_drawn, drawn, st);
     PSLAM_CUDA(c, cudaStreamSynchronize(cs));
-    PSLAM_CUDA(c, cudaStreamSynchronize(st));
+    if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
     for (int f = 0; f < nframes; ++f) {
         if (B.h_status[nframes + f] & (32 | 64)) return set_error(c, PSLAM_E_CAPACITY, "frame construct: more voxels than the plane post-processing capacity");
         if (out->n_keys[f] > cap || B.h_status[f]) return set_error(c, PSLAM_E_CAPACITY, "frame construct: ORB candidate / key point capacity exceeded");

@@ -11,20 +11,6 @@
 
 namespace pslam {
 
-struct DevVec {                       // grow-only device array
-    void* p = nullptr; size_t cap = 0;
-    int ensure(pslam_ctx* c, size_t bytes) {
-        if (bytes <= cap) return PSLAM_OK;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
-        const size_t nb = std::max<size_t>(bytes * 3 / 2, 256);
-        const int rc = check_cuda(c, cudaMalloc(&p, nb), "cudaMalloc(lba)");
-        if (rc == PSLAM_OK) cap = nb;
-        return rc;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-};
-
 struct LbaBuffers {
     int n_prob = 0;
     std::vector<LbaHeaderDev> hdr;
@@ -36,7 +22,7 @@ struct LbaBuffers {
     size_t tot_kf = 0, tot_lm = 0, tot_edges = 0, tot_col = 0, tot_flags = 0, tot_hs = 0;
     int max_smem = 0;
     // device
-    DevVec d_hdr, d_kf_Tcw0, d_kf_fixed, d_kf_K, d_kf_col, d_kf_T, d_kf_Tb, d_kf_active, d_out_Tcw, d_Hpp, d_bp, d_coeff, d_xp, d_lm_type, d_lm_val0,
+    DevArray<uint8_t> d_hdr, d_kf_Tcw0, d_kf_fixed, d_kf_K, d_kf_col, d_kf_T, d_kf_Tb, d_kf_active, d_out_Tcw, d_Hpp, d_bp, d_coeff, d_xp, d_lm_type, d_lm_val0,
         d_lm_val, d_lm_valb, d_Hll, d_bl, d_Dinv, d_db, d_xl, d_lm_active, d_edges, d_err, d_JA, d_JB, d_we, d_re, d_W, d_Y, d_level, d_o2s,
         d_kf_eoff, d_kf_eidx, d_lm_eoff, d_plane_edges, d_blk_ij, d_blk_toff, d_terms, d_hs, d_flags, d_out;
     // fetch staging
@@ -44,13 +30,6 @@ struct LbaBuffers {
     // per problem bookkeeping for fetch
     struct Shape { int n_kf, n_points, n_lines, n_planes, n_pt_obs, n_line_obs, n_plane_obs[3]; };
     std::vector<Shape> shape;
-    void release() {
-        for (DevVec* v : {&d_hdr, &d_kf_Tcw0, &d_kf_fixed, &d_kf_K, &d_kf_col, &d_kf_T, &d_kf_Tb, &d_kf_active, &d_out_Tcw, &d_Hpp, &d_bp, &d_coeff, &d_xp,
-                          &d_lm_type, &d_lm_val0, &d_lm_val, &d_lm_valb, &d_Hll, &d_bl, &d_Dinv, &d_db, &d_xl, &d_lm_active, &d_edges, &d_err, &d_JA,
-                          &d_JB, &d_we, &d_re, &d_W, &d_Y, &d_level, &d_o2s, &d_kf_eoff, &d_kf_eidx, &d_lm_eoff, &d_plane_edges, &d_blk_ij,
-                          &d_blk_toff, &d_terms, &d_hs, &d_flags, &d_out})
-            v->release();
-    }
 };
 
 static void lba_plane_from_float4(const float* v, double out[4]) {     // Converter::toPlane3D + Plane3D::normalize
@@ -234,7 +213,7 @@ int lba_pack_upload(pslam_ctx* c, const pslam_lba_problem* probs, int nprob) {
 
     // ---- device allocation + upload ----
     int rc;
-#define ENS(v, bytes) if ((rc = B.v.ensure(c, std::max<size_t>((bytes), 8))) != PSLAM_OK) return rc
+#define ENS(v, bytes) if ((rc = B.v.grow(c, std::max<size_t>((bytes), 8))) != PSLAM_OK) return rc
     ENS(d_hdr, nprob * sizeof(LbaHeaderDev)); ENS(d_out, nprob * sizeof(LbaOutDev));
     ENS(d_kf_Tcw0, B.tot_kf * 16 * 4); ENS(d_kf_fixed, B.tot_kf); ENS(d_kf_K, B.tot_kf * 5 * 8); ENS(d_kf_col, B.tot_kf * 4);
     ENS(d_kf_T, B.tot_kf * 8 * 8); ENS(d_kf_Tb, B.tot_kf * 8 * 8); ENS(d_kf_active, B.tot_kf); ENS(d_out_Tcw, B.tot_kf * 16 * 8);
@@ -250,7 +229,7 @@ int lba_pack_upload(pslam_ctx* c, const pslam_lba_problem* probs, int nprob) {
     ENS(d_terms, B.terms.size() * sizeof(int2)); ENS(d_hs, B.tot_hs * 8); ENS(d_flags, B.tot_flags);
 #undef ENS
     cudaStream_t st = c->stream;
-#define UP(v, vec) if (!(vec).empty()) PSLAM_CUDA(c, cudaMemcpyAsync(B.v.p, (vec).data(), (vec).size() * sizeof((vec)[0]), cudaMemcpyHostToDevice, st))
+#define UP(v, vec) if (!(vec).empty()) PSLAM_CUDA(c, cudaMemcpyAsync(B.v, (vec).data(), (vec).size() * sizeof((vec)[0]), cudaMemcpyHostToDevice, st))
     UP(d_hdr, B.hdr); UP(d_kf_Tcw0, B.kf_Tcw0); UP(d_kf_fixed, B.kf_fixed); UP(d_kf_K, B.kf_K); UP(d_kf_col, B.kf_col);
     UP(d_lm_type, B.lm_type); UP(d_lm_val0, B.lm_val0); UP(d_edges, B.edges); UP(d_o2s, B.orig2sorted); UP(d_kf_eoff, B.kf_edge_off);
     UP(d_kf_eidx, B.kf_edge_idx); UP(d_lm_eoff, B.lm_edge_off); UP(d_plane_edges, B.plane_edges); UP(d_blk_ij, B.blk_ij);
@@ -265,18 +244,18 @@ int lba_run_packed(pslam_ctx* c) {
     if (!c->lba || c->lba->n_prob < 1) return set_error(c, PSLAM_E_INVALID, "no packed LBA problems");
     LbaBuffers& B = *c->lba;
     LbaArrays A;
-    A.hdr = (const LbaHeaderDev*)B.d_hdr.p;
-    A.kf_Tcw0 = (const float*)B.d_kf_Tcw0.p; A.kf_fixed = (const uint8_t*)B.d_kf_fixed.p; A.kf_K = (const double*)B.d_kf_K.p; A.kf_col = (const int32_t*)B.d_kf_col.p;
-    A.kf_T = (double*)B.d_kf_T.p; A.kf_Tb = (double*)B.d_kf_Tb.p; A.kf_active = (uint8_t*)B.d_kf_active.p; A.out_Tcw = (double*)B.d_out_Tcw.p;
-    A.Hpp = (double*)B.d_Hpp.p; A.bp = (double*)B.d_bp.p; A.coeff = (double*)B.d_coeff.p; A.xp = (double*)B.d_xp.p;
-    A.lm_type = (const int32_t*)B.d_lm_type.p; A.lm_val0 = (const double*)B.d_lm_val0.p; A.lm_val = (double*)B.d_lm_val.p; A.lm_valb = (double*)B.d_lm_valb.p;
-    A.Hll = (double*)B.d_Hll.p; A.bl = (double*)B.d_bl.p; A.Dinv = (double*)B.d_Dinv.p; A.db = (double*)B.d_db.p; A.xl = (double*)B.d_xl.p;
-    A.lm_active = (uint8_t*)B.d_lm_active.p;
-    A.edges = (const LbaEdgeDev*)B.d_edges.p; A.err = (double*)B.d_err.p; A.JA = (double*)B.d_JA.p; A.JB = (double*)B.d_JB.p; A.we = (double*)B.d_we.p;
-    A.re = (double*)B.d_re.p; A.W = (double*)B.d_W.p; A.Y = (double*)B.d_Y.p; A.level = (uint8_t*)B.d_level.p; A.orig2sorted = (const int32_t*)B.d_o2s.p;
-    A.kf_edge_off = (const int32_t*)B.d_kf_eoff.p; A.kf_edge_idx = (const int32_t*)B.d_kf_eidx.p; A.lm_edge_off = (const int32_t*)B.d_lm_eoff.p;
-    A.plane_edges = (const int32_t*)B.d_plane_edges.p; A.blk_ij = (const int32_t*)B.d_blk_ij.p; A.blk_term_off = (const int32_t*)B.d_blk_toff.p;
-    A.terms = (const int2*)B.d_terms.p; A.hs_global = (double*)B.d_hs.p; A.flags = (uint8_t*)B.d_flags.p; A.out = (LbaOutDev*)B.d_out.p;
+    A.hdr = (const LbaHeaderDev*)B.d_hdr.ptr;
+    A.kf_Tcw0 = (const float*)B.d_kf_Tcw0.ptr; A.kf_fixed = (const uint8_t*)B.d_kf_fixed.ptr; A.kf_K = (const double*)B.d_kf_K.ptr; A.kf_col = (const int32_t*)B.d_kf_col.ptr;
+    A.kf_T = (double*)B.d_kf_T.ptr; A.kf_Tb = (double*)B.d_kf_Tb.ptr; A.kf_active = (uint8_t*)B.d_kf_active.ptr; A.out_Tcw = (double*)B.d_out_Tcw.ptr;
+    A.Hpp = (double*)B.d_Hpp.ptr; A.bp = (double*)B.d_bp.ptr; A.coeff = (double*)B.d_coeff.ptr; A.xp = (double*)B.d_xp.ptr;
+    A.lm_type = (const int32_t*)B.d_lm_type.ptr; A.lm_val0 = (const double*)B.d_lm_val0.ptr; A.lm_val = (double*)B.d_lm_val.ptr; A.lm_valb = (double*)B.d_lm_valb.ptr;
+    A.Hll = (double*)B.d_Hll.ptr; A.bl = (double*)B.d_bl.ptr; A.Dinv = (double*)B.d_Dinv.ptr; A.db = (double*)B.d_db.ptr; A.xl = (double*)B.d_xl.ptr;
+    A.lm_active = (uint8_t*)B.d_lm_active.ptr;
+    A.edges = (const LbaEdgeDev*)B.d_edges.ptr; A.err = (double*)B.d_err.ptr; A.JA = (double*)B.d_JA.ptr; A.JB = (double*)B.d_JB.ptr; A.we = (double*)B.d_we.ptr;
+    A.re = (double*)B.d_re.ptr; A.W = (double*)B.d_W.ptr; A.Y = (double*)B.d_Y.ptr; A.level = (uint8_t*)B.d_level.ptr; A.orig2sorted = (const int32_t*)B.d_o2s.ptr;
+    A.kf_edge_off = (const int32_t*)B.d_kf_eoff.ptr; A.kf_edge_idx = (const int32_t*)B.d_kf_eidx.ptr; A.lm_edge_off = (const int32_t*)B.d_lm_eoff.ptr;
+    A.plane_edges = (const int32_t*)B.d_plane_edges.ptr; A.blk_ij = (const int32_t*)B.d_blk_ij.ptr; A.blk_term_off = (const int32_t*)B.d_blk_toff.ptr;
+    A.terms = (const int2*)B.d_terms.ptr; A.hs_global = (double*)B.d_hs.ptr; A.flags = (uint8_t*)B.d_flags.ptr; A.out = (LbaOutDev*)B.d_out.ptr;
     // per device and cheap: set on every launch (contexts of one process may live on different GPUs)
     PSLAM_CUDA(c, cudaFuncSetAttribute(k_local_bundle_adjustment, cudaFuncAttributeMaxDynamicSharedMemorySize, LBA_SMEM_BUDGET));
     PSLAM_LAUNCH(c, "local_bundle_adjustment", k_local_bundle_adjustment<<<B.n_prob, LBA_THREADS, B.max_smem, c->stream>>>(A));
@@ -289,10 +268,10 @@ int lba_fetch(pslam_ctx* c, pslam_lba_result* res) {
     LbaBuffers& B = *c->lba;
     B.h_Tcw.resize(B.tot_kf * 16); B.h_lm.resize(B.tot_lm * 4); B.h_flags.resize(std::max<size_t>(B.tot_flags, 1)); B.h_out.resize(B.n_prob);
     cudaStream_t st = c->stream;
-    PSLAM_CUDA(c, cudaMemcpyAsync(B.h_Tcw.data(), B.d_out_Tcw.p, B.tot_kf * 16 * 8, cudaMemcpyDeviceToHost, st));
-    if (B.tot_lm) PSLAM_CUDA(c, cudaMemcpyAsync(B.h_lm.data(), B.d_lm_val.p, B.tot_lm * 4 * 8, cudaMemcpyDeviceToHost, st));
-    if (B.tot_flags) PSLAM_CUDA(c, cudaMemcpyAsync(B.h_flags.data(), B.d_flags.p, B.tot_flags, cudaMemcpyDeviceToHost, st));
-    PSLAM_CUDA(c, cudaMemcpyAsync(B.h_out.data(), B.d_out.p, B.n_prob * sizeof(LbaOutDev), cudaMemcpyDeviceToHost, st));
+    PSLAM_CUDA(c, cudaMemcpyAsync(B.h_Tcw.data(), B.d_out_Tcw.ptr, B.tot_kf * 16 * 8, cudaMemcpyDeviceToHost, st));
+    if (B.tot_lm) PSLAM_CUDA(c, cudaMemcpyAsync(B.h_lm.data(), B.d_lm_val.ptr, B.tot_lm * 4 * 8, cudaMemcpyDeviceToHost, st));
+    if (B.tot_flags) PSLAM_CUDA(c, cudaMemcpyAsync(B.h_flags.data(), B.d_flags.ptr, B.tot_flags, cudaMemcpyDeviceToHost, st));
+    PSLAM_CUDA(c, cudaMemcpyAsync(B.h_out.data(), B.d_out.ptr, B.n_prob * sizeof(LbaOutDev), cudaMemcpyDeviceToHost, st));
     PSLAM_CUDA(c, cudaStreamSynchronize(st));
     for (int p = 0; p < B.n_prob; ++p) {
         const LbaHeaderDev& H = B.hdr[p];
@@ -336,8 +315,6 @@ int lba_fetch(pslam_ctx* c, pslam_lba_result* res) {
 }
 
 void lba_free(pslam_ctx* c) {
-    if (!c->lba) return;
-    c->lba->release();
     delete c->lba;
     c->lba = nullptr;
 }

@@ -299,27 +299,24 @@ int pslam_lines3d_batch(pslam_ctx* c, const pslam_keyline* keylines, const int32
         return set_error(c, PSLAM_E_INVALID, "bad lines3d arguments");
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     cudaStream_t st = c->stream;
-    const size_t npx = (size_t)c->cfg.width * c->cfg.height;
-    const size_t sz[] = {(size_t)nframes * max_lines * sizeof(pslam_keyline), (size_t)nframes * 4, (size_t)nframes * npx * 2, (size_t)nframes * 4, (size_t)nframes * 4,
-                         (size_t)nframes * max_lines * sizeof(pslam_line3d), (size_t)nframes * 4};
-    const void* src[] = {keylines, n_lines, depth, seed, skip, nullptr, nullptr};
-    size_t off[8]; off[0] = 0;
-    for (int i = 0; i < 7; ++i) off[i + 1] = (off[i] + sz[i] + 255) & ~(size_t)255;
-    uint8_t* d = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&d, off[7]));
-    cudaError_t e = cudaSuccess;
-    for (int i = 0; i < 5 && e == cudaSuccess; ++i)
-        if (src[i]) e = cudaMemcpyAsync(d + off[i], src[i], sz[i], cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) { cudaFree(d); return check_cuda(c, e, "lines3d upload"); }
-    const int rc = lines3d_launch(c, (const pslam_keyline*)(d + off[0]), (const int32_t*)(d + off[1]), max_lines, (const uint16_t*)(d + off[2]), nframes, depth_factor, cam,
-                                  (const uint32_t*)(d + off[3]), skip ? (const int32_t*)(d + off[4]) : nullptr, (pslam_line3d*)(d + off[5]), (int32_t*)(d + off[6]));
-    if (rc != PSLAM_OK) { cudaFree(d); return rc; }
-    e = cudaMemcpyAsync(out, d + off[5], sz[5], cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(n_drawn, d + off[6], sz[6], cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    if (e != cudaSuccess) return check_cuda(c, e, "lines3d");
-    return PSLAM_OK;
+    const size_t npx = (size_t)c->cfg.width * c->cfg.height, nf = (size_t)nframes;
+    Slab s;
+    const auto d_kl = s.add<pslam_keyline>(nf * max_lines);
+    const auto d_n_lines = s.add<int32_t>(nf);
+    const auto d_depth = s.add<uint16_t>(nf * npx);
+    const auto d_seed = s.add<uint32_t>(nf);
+    const auto d_skip = s.add<int32_t>(nf);
+    const auto d_out = s.add<pslam_line3d>(nf * max_lines);
+    const auto d_n_drawn = s.add<int32_t>(nf);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    s.up(d_kl, keylines, st); s.up(d_n_lines, n_lines, st); s.up(d_depth, depth, st); s.up(d_seed, seed, st);
+    if (skip) s.up(d_skip, skip, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    rc = lines3d_launch(c, s[d_kl], s[d_n_lines], max_lines, s[d_depth], nframes, depth_factor, cam, s[d_seed], skip ? s[d_skip] : nullptr, s[d_out], s[d_n_drawn]);
+    if (rc != PSLAM_OK) return rc;
+    s.down(out, d_out, st); s.down(n_drawn, d_n_drawn, st);
+    return s.sync(c, st);
 }
 
 }

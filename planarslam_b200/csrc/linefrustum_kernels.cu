@@ -43,23 +43,23 @@ extern "C" int pslam_lines_in_frustum(pslam_ctx* c, const pslam_line_frustum_fra
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     cudaStream_t st = c->stream;
     const size_t N = (size_t)n;
-    const size_t sz[] = {N * 48, N * 24, N * 4, N * 4, N, N * 16, N * 4, N * 4, 4};
-    const void* src[] = {pos, normal, max_distance, min_distance};
-    size_t off[10]; off[0] = 0;
-    for (int i = 0; i < 9; ++i) off[i + 1] = (off[i] + sz[i] + 255) & ~(size_t)255;
-    uint8_t* d = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&d, off[9]));
-    cudaError_t e = cudaMemsetAsync(d + off[8], 0, 4, st);
-    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaMemcpyAsync(d + off[i], src[i], sz[i], cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) { cudaFree(d); return check_cuda(c, e, "line frustum upload"); }
-    PSLAM_LAUNCH(c, "lines_in_frustum", k_lines_in_frustum<<<(n + 127) / 128, 128, 0, st>>>(F, n, (const double*)(d + off[0]), (const double*)(d + off[1]),
-                 (const float*)(d + off[2]), (const float*)(d + off[3]), cos_limit, d + off[4], (float*)(d + off[5]), (int32_t*)(d + off[6]), (float*)(d + off[7]),
-                 (int32_t*)(d + off[8])));
+    Slab s;
+    const auto d_pos = s.add<double>(N * 6), d_normal = s.add<double>(N * 3);
+    const auto d_max_d = s.add<float>(N), d_min_d = s.add<float>(N);
+    const auto d_in_view = s.add<uint8_t>(N);
+    const auto d_proj = s.add<float>(N * 4);
+    const auto d_level = s.add<int32_t>(N);
+    const auto d_view_cos = s.add<float>(N);
+    const auto d_cnt = s.add<int32_t>(1);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    s.zero(d_cnt, st);
+    s.up(d_pos, pos, st); s.up(d_normal, normal, st); s.up(d_max_d, max_distance, st); s.up(d_min_d, min_distance, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    PSLAM_LAUNCH(c, "lines_in_frustum", k_lines_in_frustum<<<(n + 127) / 128, 128, 0, st>>>(F, n, s[d_pos], s[d_normal], s[d_max_d], s[d_min_d], cos_limit, s[d_in_view],
+                 s[d_proj], s[d_level], s[d_view_cos], s[d_cnt]));
     int32_t cnt = 0;
-    void* dst[] = {in_view, proj, level, view_cos, &cnt};
-    for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = cudaMemcpyAsync(dst[i], d + off[4 + i], sz[4 + i], cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    if (e != cudaSuccess) return check_cuda(c, e, "line frustum");
+    s.down(in_view, d_in_view, st); s.down(proj, d_proj, st); s.down(level, d_level, st); s.down(view_cos, d_view_cos, st); s.down(&cnt, d_cnt, st);
+    if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
     return cnt;
 }

@@ -96,22 +96,25 @@ extern "C" int pslam_line_search_by_projection(pslam_ctx* c, int nf, const float
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     cudaStream_t st = c->stream;
     // small POD arrays: one staging allocation per call (a live tracker calls this once per frame)
-    const size_t sz[] = {(size_t)nf * 8, (size_t)nf * 4, (size_t)nf * 4, (size_t)nf * 32, (size_t)nf, (size_t)n_levels * 4, (size_t)nm, (size_t)nm * 4,
-                         (size_t)nm * 4, (size_t)nm * 16, (size_t)nm * 32, (size_t)nm, (size_t)nf * 4, 4};
-    const void* src[] = {pt, angle, octave, desc, has_obs, scale_factors, skip, level, view_cos, proj, mdesc, m_has_obs, nullptr, nullptr};
-    size_t off[15]; off[0] = 0;
-    for (int i = 0; i < 14; ++i) off[i + 1] = (off[i] + sz[i] + 15) & ~(size_t)15;
-    uint8_t* d = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&d, off[14]));
-    for (int i = 0; i < 12; ++i) if (sz[i]) { const cudaError_t e = cudaMemcpyAsync(d + off[i], src[i], sz[i], cudaMemcpyHostToDevice, st); if (e != cudaSuccess) { cudaFree(d); return check_cuda(c, e, "line search upload"); } }
-    PSLAM_LAUNCH(c, "line_search", k_line_search<<<1, 32, 0, st>>>(nf, (const float*)(d + off[0]), (const float*)(d + off[1]), (const int32_t*)(d + off[2]), d + off[3],
-                 d + off[4], (const float*)(d + off[5]), n_levels, nm, d + off[6], (const int32_t*)(d + off[7]), (const float*)(d + off[8]), (const float*)(d + off[9]),
-                 d + off[10], d + off[11], th, nnratio, (int32_t*)(d + off[12]), (int32_t*)(d + off[13])));
+    Slab s;
+    const auto d_pt = s.add<float>((size_t)nf * 2), d_angle = s.add<float>(nf);
+    const auto d_octave = s.add<int32_t>(nf);
+    const auto d_desc = s.add<uint8_t>((size_t)nf * 32), d_has_obs = s.add<uint8_t>(nf);
+    const auto d_scale = s.add<float>(n_levels);
+    const auto d_skip = s.add<uint8_t>(nm);
+    const auto d_level = s.add<int32_t>(nm);
+    const auto d_view_cos = s.add<float>(nm), d_proj = s.add<float>((size_t)nm * 4);
+    const auto d_mdesc = s.add<uint8_t>((size_t)nm * 32), d_m_has_obs = s.add<uint8_t>(nm);
+    const auto d_assigned = s.add<int32_t>(nf), d_n = s.add<int32_t>(1);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    s.up(d_pt, pt, st); s.up(d_angle, angle, st); s.up(d_octave, octave, st); s.up(d_desc, desc, st); s.up(d_has_obs, has_obs, st); s.up(d_scale, scale_factors, st);
+    s.up(d_skip, skip, st); s.up(d_level, level, st); s.up(d_view_cos, view_cos, st); s.up(d_proj, proj, st); s.up(d_mdesc, mdesc, st); s.up(d_m_has_obs, m_has_obs, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    PSLAM_LAUNCH(c, "line_search", k_line_search<<<1, 32, 0, st>>>(nf, s[d_pt], s[d_angle], s[d_octave], s[d_desc], s[d_has_obs], s[d_scale], n_levels, nm, s[d_skip],
+                 s[d_level], s[d_view_cos], s[d_proj], s[d_mdesc], s[d_m_has_obs], th, nnratio, s[d_assigned], s[d_n]));
     int32_t n = 0;
-    cudaError_t e = cudaMemcpyAsync(assigned, d + off[12], (size_t)nf * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&n, d + off[13], 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    if (e != cudaSuccess) return check_cuda(c, e, "line search");
+    s.down(assigned, d_assigned, st); s.down(&n, d_n, st);
+    if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
     return n;
 }

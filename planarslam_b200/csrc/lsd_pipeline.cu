@@ -5,6 +5,7 @@
 #include <cmath>
 #include <cstring>
 #include <cstdlib>
+#include <memory>
 #include <string>
 
 #include "lsd_kernels.cuh"
@@ -14,17 +15,17 @@ namespace pslam {
 
 struct LsdBuffers {
     LsdGeom g;
-    int max_batch = 0, last_n = 0, max_lines_cap = 0;
-    int16_t *d_ix = nullptr, *d_ax = nullptr, *d_iy = nullptr, *d_ay = nullptr;
-    float2* d_lut = nullptr; double* d_lgamma = nullptr; double* d_nfa = nullptr;
-    uint8_t* d_gray = nullptr;        // staging for the host-pointer entry points
-    uint8_t* d_scaled = nullptr; uint32_t* d_ang = nullptr; float2* d_cs = nullptr; uint32_t* d_gxy = nullptr; int32_t* d_smax = nullptr;
-    uint32_t* d_reg = nullptr; uint32_t* d_order = nullptr; int32_t* d_norder = nullptr;
-    double* d_cands = nullptr; double* d_cand_nfa = nullptr; int32_t* d_ncand = nullptr;
-    uint32_t* d_fail = nullptr; int32_t* d_nfail = nullptr;      // candidates whose first NFA evaluation fails (queue of k_lsd_improve)
-    float4* d_segs = nullptr; double* d_wpn = nullptr; int32_t* d_nsegs = nullptr; int32_t* d_status = nullptr;
-    LsdKeyLine* d_kl = nullptr; double* d_lf = nullptr; int32_t* d_nkl = nullptr;
-    int16_t *d_dx = nullptr, *d_dy = nullptr; float *d_glocal = nullptr, *d_gglobal = nullptr; uint8_t* d_ldesc = nullptr; float* d_lbd72 = nullptr;   // LBD (lbd_kernels.cuh)
+    int max_batch = 0, last_n = 0;
+    DevArray<int16_t> d_ix, d_ax, d_iy, d_ay;
+    DevArray<float2> d_lut; DevArray<double> d_lgamma, d_nfa;
+    DevArray<uint8_t> d_gray;         // staging for the host-pointer entry points
+    DevArray<uint8_t> d_scaled; DevArray<uint32_t> d_ang; DevArray<float2> d_cs; DevArray<uint32_t> d_gxy; DevArray<int32_t> d_smax;
+    DevArray<uint32_t> d_reg, d_order; DevArray<int32_t> d_norder;
+    DevArray<double> d_cands, d_cand_nfa; DevArray<int32_t> d_ncand;
+    DevArray<uint32_t> d_fail; DevArray<int32_t> d_nfail;      // candidates whose first NFA evaluation fails (queue of k_lsd_improve)
+    DevArray<float4> d_segs; DevArray<double> d_wpn; DevArray<int32_t> d_nsegs, d_status;
+    DevArray<LsdKeyLine> d_kl; DevArray<double> d_lf; DevArray<int32_t> d_nkl;
+    DevArray<int16_t> d_dx, d_dy; DevArray<float> d_glocal, d_gglobal; DevArray<uint8_t> d_ldesc; DevArray<float> d_lbd72;   // LBD (lbd_kernels.cuh)
     std::vector<int32_t> h_n, h_status;
 };
 
@@ -49,13 +50,13 @@ static const int LSD_SEG_CAP = 4096;
 
 int lsd_alloc(pslam_ctx* c) {
     if (c->lsd) return PSLAM_OK;
-    LsdBuffers* Bp = new LsdBuffers();
+    std::unique_ptr<LsdBuffers> Bp(new LsdBuffers());
     LsdBuffers& B = *Bp;
     LsdGeom& g = B.g;
     g.w = c->cfg.width; g.h = c->cfg.height;
     const double SCALE = 0.8, ANG_TH = 22.5, QUANT = 2.0;
     g.W = lsd_cv_round(g.w * SCALE); g.H = lsd_cv_round(g.h * SCALE);
-    if (g.W < 8 || g.H < 8 || g.W > 32767 || g.H > 32767) { delete Bp; return set_error(c, PSLAM_E_INVALID, "image size unsupported by the line-segment detector"); }
+    if (g.W < 8 || g.H < 8 || g.W > 32767 || g.H > 32767) return set_error(c, PSLAM_E_INVALID, "image size unsupported by the line-segment detector");
     g.refine = 2;
     // candidate / segment capacity per frame: 4096 at 640x480 (a textured frame yields a few hundred), scaled with the image area above that
     g.seg_cap = g.cand_cap = std::max(LSD_SEG_CAP, (int)(((long long)LSD_SEG_CAP * g.w * g.h / (640 * 480) + 1023) / 1024 * 1024));
@@ -89,11 +90,11 @@ int lsd_alloc(pslam_ctx* c) {
     // the blur / scale kernel stages (tile * 1.25 + 6) source pixels: check the compiled bounds
     for (int X0 = 0; X0 < g.W; X0 += LSD_TW) {
         const int X1 = std::min(X0 + LSD_TW, g.W) - 1;
-        if (std::min(ix[X1] + 1, g.w - 1) - ix[X0] + 5 > LSD_SW) { delete Bp; return set_error(c, PSLAM_E_INVALID, "LSD tile bound (width)"); }
+        if (std::min(ix[X1] + 1, g.w - 1) - ix[X0] + 5 > LSD_SW) return set_error(c, PSLAM_E_INVALID, "LSD tile bound (width)");
     }
     for (int Y0 = 0; Y0 < g.H; Y0 += LSD_TH) {
         const int Y1 = std::min(Y0 + LSD_TH, g.H) - 1;
-        if (std::min(iy[Y1] + 1, g.h - 1) - iy[Y0] + 5 > LSD_SH) { delete Bp; return set_error(c, PSLAM_E_INVALID, "LSD tile bound (height)"); }
+        if (std::min(iy[Y1] + 1, g.h - 1) - iy[Y0] + 5 > LSD_SH) return set_error(c, PSLAM_E_INVALID, "LSD tile bound (height)");
     }
     // cosf / sinf of the level-line angle for every possible gradient: the float sums of region_grow use libm's float routines
     std::vector<float2> lut((size_t)1021 * 1021);
@@ -116,15 +117,16 @@ int lsd_alloc(pslam_ctx* c) {
         }
     }
     const size_t npx = (size_t)g.W * g.H, nb = (size_t)B.max_batch;
-#define LA(ptr, bytes) do { const int rc_ = check_cuda(c, cudaMalloc((void**)&(ptr), (bytes)), "cudaMalloc(lsd)"); if (rc_ != PSLAM_OK) { c->lsd = Bp; lsd_free(c); return rc_; } } while (0)
-    LA(B.d_ix, g.W * 2); LA(B.d_ax, g.W * 2); LA(B.d_iy, g.H * 2); LA(B.d_ay, g.H * 2); LA(B.d_lut, lut.size() * sizeof(float2)); LA(B.d_lgamma, LSD_LGAMMA_N * 8);
-    LA(B.d_nfa, (size_t)LSD_NFA_NJ * LSD_NFA_TRI * 8);
-    LA(B.d_gray, nb * g.w * g.h); LA(B.d_scaled, nb * npx); LA(B.d_ang, nb * npx * 4); LA(B.d_cs, nb * npx * 8); LA(B.d_gxy, nb * npx * 4); LA(B.d_smax, nb * 4);
-    LA(B.d_reg, nb * npx * 4); LA(B.d_order, nb * npx * 4); LA(B.d_norder, nb * 4);
-    LA(B.d_fail, nb * g.cand_cap * 4); LA(B.d_nfail, nb * 4);
-    LA(B.d_cands, nb * g.cand_cap * 12 * 8); LA(B.d_cand_nfa, nb * g.cand_cap * 8); LA(B.d_ncand, nb * 4);
-    LA(B.d_segs, nb * g.seg_cap * sizeof(float4)); LA(B.d_wpn, nb * g.seg_cap * 3 * 8); LA(B.d_nsegs, nb * 4); LA(B.d_status, nb * 4);
-#undef LA
+    int rc;
+    if ((rc = B.d_ix.reserve(c, g.W)) || (rc = B.d_ax.reserve(c, g.W)) || (rc = B.d_iy.reserve(c, g.H)) || (rc = B.d_ay.reserve(c, g.H)) ||
+        (rc = B.d_lut.reserve(c, lut.size())) || (rc = B.d_lgamma.reserve(c, LSD_LGAMMA_N)) || (rc = B.d_nfa.reserve(c, (size_t)LSD_NFA_NJ * LSD_NFA_TRI)) ||
+        (rc = B.d_gray.reserve(c, nb * g.w * g.h)) || (rc = B.d_scaled.reserve(c, nb * npx)) || (rc = B.d_ang.reserve(c, nb * npx)) || (rc = B.d_cs.reserve(c, nb * npx)) ||
+        (rc = B.d_gxy.reserve(c, nb * npx)) || (rc = B.d_smax.reserve(c, nb)) ||
+        (rc = B.d_reg.reserve(c, nb * npx)) || (rc = B.d_order.reserve(c, nb * npx)) || (rc = B.d_norder.reserve(c, nb)) ||
+        (rc = B.d_fail.reserve(c, nb * g.cand_cap)) || (rc = B.d_nfail.reserve(c, nb)) ||
+        (rc = B.d_cands.reserve(c, nb * g.cand_cap * 12)) || (rc = B.d_cand_nfa.reserve(c, nb * g.cand_cap)) || (rc = B.d_ncand.reserve(c, nb)) ||
+        (rc = B.d_segs.reserve(c, nb * g.seg_cap)) || (rc = B.d_wpn.reserve(c, nb * g.seg_cap * 3)) || (rc = B.d_nsegs.reserve(c, nb)) || (rc = B.d_status.reserve(c, nb)))
+        return rc;
     cudaStream_t st = c->stream;
     PSLAM_CUDA(c, cudaMemcpyAsync(B.d_ix, ix.data(), g.W * 2, cudaMemcpyHostToDevice, st));
     PSLAM_CUDA(c, cudaMemcpyAsync(B.d_ax, ax.data(), g.W * 2, cudaMemcpyHostToDevice, st));
@@ -138,18 +140,11 @@ int lsd_alloc(pslam_ctx* c) {
     k_lsd_nfa_table<<<(LSD_NFA_NJ * LSD_NFA_TRI + 255) / 256, 256, 0, st>>>(g, B.d_nfa);
     PSLAM_CUDA(c, cudaGetLastError());
     PSLAM_CUDA(c, cudaStreamSynchronize(st));
-    c->lsd = Bp;
+    c->lsd = Bp.release();
     return PSLAM_OK;
 }
 
 void lsd_free(pslam_ctx* c) {
-    if (!c->lsd) return;
-    LsdBuffers& B = *c->lsd;
-    for (void* p : {(void*)B.d_ix, (void*)B.d_ax, (void*)B.d_iy, (void*)B.d_ay, (void*)B.d_lut, (void*)B.d_lgamma, (void*)B.d_nfa, (void*)B.d_gray, (void*)B.d_scaled, (void*)B.d_ang, (void*)B.d_cs, (void*)B.d_gxy,
-                    (void*)B.d_smax, (void*)B.d_reg, (void*)B.d_order, (void*)B.d_norder, (void*)B.d_segs, (void*)B.d_wpn,
-                    (void*)B.d_nsegs, (void*)B.d_status, (void*)B.d_cands, (void*)B.d_cand_nfa, (void*)B.d_ncand, (void*)B.d_fail, (void*)B.d_nfail, (void*)B.d_kl, (void*)B.d_lf, (void*)B.d_nkl, (void*)B.d_dx, (void*)B.d_dy, (void*)B.d_glocal, (void*)B.d_gglobal,
-                    (void*)B.d_ldesc, (void*)B.d_lbd72})
-        if (p) cudaFree(p);
     delete c->lsd;
     c->lsd = nullptr;
 }
@@ -272,19 +267,11 @@ int pslam_lsd_detect_batch(pslam_ctx* c, const uint8_t* gray, int nframes, int r
 
 static int lsd_ensure_kl(pslam_ctx* c, int max_lines) {
     LsdBuffers& B = *c->lsd;
-    if (max_lines <= B.max_lines_cap) return PSLAM_OK;
-    if (B.d_kl) cudaFree(B.d_kl);
-    if (B.d_lf) cudaFree(B.d_lf);
-    if (B.d_nkl) cudaFree(B.d_nkl);
-    if (B.d_ldesc) cudaFree(B.d_ldesc);
-    if (B.d_lbd72) cudaFree(B.d_lbd72);
-    B.d_kl = nullptr; B.d_lf = nullptr; B.d_nkl = nullptr; B.d_ldesc = nullptr; B.d_lbd72 = nullptr; B.max_lines_cap = 0;
-    PSLAM_CUDA(c, cudaMalloc((void**)&B.d_kl, (size_t)B.max_batch * max_lines * sizeof(LsdKeyLine)));
-    PSLAM_CUDA(c, cudaMalloc((void**)&B.d_lf, (size_t)B.max_batch * max_lines * 24));
-    PSLAM_CUDA(c, cudaMalloc((void**)&B.d_nkl, (size_t)B.max_batch * 4));
-    PSLAM_CUDA(c, cudaMalloc((void**)&B.d_ldesc, (size_t)B.max_batch * max_lines * 32));
-    PSLAM_CUDA(c, cudaMalloc((void**)&B.d_lbd72, (size_t)B.max_batch * max_lines * 72 * 4));
-    B.max_lines_cap = max_lines;
+    const size_t n = (size_t)B.max_batch * max_lines;
+    int rc;
+    if ((rc = B.d_kl.reserve(c, n)) || (rc = B.d_lf.reserve(c, n * 3)) || (rc = B.d_nkl.reserve(c, B.max_batch)) || (rc = B.d_ldesc.reserve(c, n * 32)) ||
+        (rc = B.d_lbd72.reserve(c, n * 72)))
+        return rc;
     return PSLAM_OK;
 }
 
@@ -293,10 +280,11 @@ static int lbd_describe_dev(pslam_ctx* c, const uint8_t* d_gray, int nframes, in
     LsdBuffers& B = *c->lsd;
     const LsdGeom& g = B.g;
     cudaStream_t st = c->stream;
-    if (!B.d_dx) {
-        const size_t bytes = (size_t)B.max_batch * g.w * g.h * sizeof(int16_t);
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_dx, bytes)); PSLAM_CUDA(c, cudaMalloc((void**)&B.d_dy, bytes));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_glocal, LBD_WIDTH * 3 * 4)); PSLAM_CUDA(c, cudaMalloc((void**)&B.d_gglobal, LBD_HEIGHT * 4));
+    if (!B.d_gglobal) {                                        // first call: the gradient planes and the two Gaussian windows
+        const size_t px = (size_t)B.max_batch * g.w * g.h;
+        int rc;
+        if ((rc = B.d_dx.reserve(c, px)) || (rc = B.d_dy.reserve(c, px)) || (rc = B.d_glocal.reserve(c, LBD_WIDTH * 3)) || (rc = B.d_gglobal.reserve(c, LBD_HEIGHT)))
+            return rc;
         float gl[LBD_WIDTH * 3], gg[LBD_HEIGHT];               // the two Gaussian windows, evaluated with the host libm like upstream (integer-division sigmas)
         { const double u = (double)((LBD_WIDTH * 3 - 1) / 2), sigma = (double)((LBD_WIDTH * 2 + 1) / 2), inv = -1 / (2 * sigma * sigma);
           for (int i = 0; i < LBD_WIDTH * 3; ++i) { const double d = i - u; gl[i] = (float)std::exp(d * d * inv); } }

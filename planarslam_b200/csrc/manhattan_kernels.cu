@@ -196,25 +196,22 @@ int pslam_track_manhattan_batch(pslam_ctx* c, const float* R_last, const float* 
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     cudaStream_t st = c->stream;
     const size_t nf = (size_t)nframes;
-    const size_t sz[] = {nf * 36, nf * max_normals * 12, nf * 4, nf * max_dirs * 24, nf * 4, nf * sizeof(pslam_manhattan_result), nf * max_normals, nf * max_dirs};
-    const void* src[] = {R_last, normals, n_normals, dirs, n_dirs, nullptr, nullptr, nullptr};
-    void* dst[] = {nullptr, nullptr, nullptr, nullptr, nullptr, res, normal_mask, dir_mask};
-    size_t off[9]; off[0] = 0;
-    for (int i = 0; i < 8; ++i) off[i + 1] = (off[i] + sz[i] + 255) & ~(size_t)255;
-    uint8_t* d = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&d, off[8]));
-    cudaError_t e = cudaSuccess;
-    for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = cudaMemcpyAsync(d + off[i], src[i], sz[i], cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) { cudaFree(d); return check_cuda(c, e, "manhattan upload"); }
-    const int rc = pslam_track_manhattan_batch_dev(c, (const float*)(d + off[0]), (const float*)(d + off[1]), (const int32_t*)(d + off[2]), max_normals,
-                                                   (const double*)(d + off[3]), (const int32_t*)(d + off[4]), max_dirs, nframes, (pslam_manhattan_result*)(d + off[5]),
-                                                   d + off[6], d + off[7]);
-    if (rc != PSLAM_OK) { cudaFree(d); return rc; }
-    for (int i = 5; i < 8 && e == cudaSuccess; ++i) e = cudaMemcpyAsync(dst[i], d + off[i], sz[i], cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    if (e != cudaSuccess) return check_cuda(c, e, "manhattan");
-    return PSLAM_OK;
+    Slab s;
+    const auto d_R = s.add<float>(nf * 9), d_normals = s.add<float>(nf * max_normals * 3);
+    const auto d_n_normals = s.add<int32_t>(nf);
+    const auto d_dirs = s.add<double>(nf * max_dirs * 3);
+    const auto d_n_dirs = s.add<int32_t>(nf);
+    const auto d_res = s.add<pslam_manhattan_result>(nf);
+    const auto d_normal_mask = s.add<uint8_t>(nf * max_normals), d_dir_mask = s.add<uint8_t>(nf * max_dirs);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    s.up(d_R, R_last, st); s.up(d_normals, normals, st); s.up(d_n_normals, n_normals, st); s.up(d_dirs, dirs, st); s.up(d_n_dirs, n_dirs, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    rc = pslam_track_manhattan_batch_dev(c, s[d_R], s[d_normals], s[d_n_normals], max_normals, s[d_dirs], s[d_n_dirs], max_dirs, nframes, s[d_res], s[d_normal_mask],
+                                         s[d_dir_mask]);
+    if (rc != PSLAM_OK) return rc;
+    s.down(res, d_res, st); s.down(normal_mask, d_normal_mask, st); s.down(dir_mask, d_dir_mask, st);
+    return s.sync(c, st);
 }
 
 }

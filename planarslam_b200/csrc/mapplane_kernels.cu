@@ -105,27 +105,25 @@ extern "C" int pslam_map_plane_update_batch(pslam_ctx* c, int n_jobs, const int3
     if ((n_pts && !pts) || (n_clouds && !T)) return set_error(c, PSLAM_E_INVALID, "bad MapPlane update arrays");
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     cudaStream_t st = c->stream;
-    const size_t sz[] = {(size_t)(n_jobs + 1) * 4, (size_t)(n_clouds + 1) * 4, (size_t)n_pts * 12, (size_t)n_clouds * 128, (size_t)n_jobs * cap * 12, (size_t)n_jobs * 4, 4};
-    const void* src[] = {job_cloud_off, cloud_pt_off, pts, T};
-    size_t off[8]; off[0] = 0;
-    for (int i = 0; i < 7; ++i) off[i + 1] = (off[i] + sz[i] + 15) & ~(size_t)15;
-    uint8_t* d = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&d, off[7]));
-    cudaError_t e = cudaMemsetAsync(d + off[6], 0, 4, st);
-    for (int i = 0; i < 4 && e == cudaSuccess; ++i) if (sz[i]) e = cudaMemcpyAsync(d + off[i], src[i], sz[i], cudaMemcpyHostToDevice, st);
+    Slab s;
+    const auto d_job_off = s.add<int32_t>(n_jobs + 1), d_cloud_off = s.add<int32_t>(n_clouds + 1);
+    const auto d_pts = s.add<float>((size_t)n_pts * 3);
+    const auto d_T = s.add<double>((size_t)n_clouds * 16);
+    const auto d_out = s.add<float>((size_t)n_jobs * cap * 3);
+    const auto d_n_out = s.add<int32_t>(n_jobs), d_flag = s.add<int32_t>(1);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    s.zero(d_flag, st);
+    s.up(d_job_off, job_cloud_off, st); s.up(d_cloud_off, cloud_pt_off, st); s.up(d_pts, pts, st); s.up(d_T, T, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
     const size_t smem = (size_t)MP_SLOTS * (3 * 8 + 3 * 4);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_map_plane_update, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { cudaFree(d); return check_cuda(c, e, "MapPlane update upload"); }
-    PSLAM_LAUNCH(c, "map_plane_update", k_map_plane_update<<<n_jobs, MP_THREADS, smem, st>>>((const int32_t*)(d + off[0]), (const int32_t*)(d + off[1]), (const float*)(d + off[2]),
-                 (const double*)(d + off[3]), cap, (float*)(d + off[4]), (int32_t*)(d + off[5]), (int32_t*)(d + off[6])));
+    PSLAM_CUDA(c, cudaFuncSetAttribute(k_map_plane_update, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PSLAM_LAUNCH(c, "map_plane_update", k_map_plane_update<<<n_jobs, MP_THREADS, smem, st>>>(s[d_job_off], s[d_cloud_off], s[d_pts], s[d_T], cap, s[d_out], s[d_n_out],
+                 s[d_flag]));
+    PSLAM_CUDA(c, cudaGetLastError());
     int32_t flag = 0;
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_pts, d + off[4], sz[4], cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(n_out, d + off[5], sz[5], cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&flag, d + off[6], 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    if (e != cudaSuccess) return check_cuda(c, e, "MapPlane update");
+    s.down(out_pts, d_out, st); s.down(n_out, d_n_out, st); s.down(&flag, d_flag, st);
+    if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
     if (flag) return set_error(c, PSLAM_E_CAPACITY, "MapPlane update: more occupied voxels than the capacity (or a point beyond the voxel key range)");
     return PSLAM_OK;
 }

@@ -132,29 +132,26 @@ int pslam_hamming_knn2(pslam_ctx* c, const uint8_t* q, int nq, const uint8_t* t,
     if (nq < 0 || nt < 0 || nt > 65535 || (nq && !q) || (nt && !t) || !idx2 || !dist2) return set_error(c, PSLAM_E_INVALID, "bad descriptor arrays");
     if (nq == 0) { if (n_good) *n_good = 0; return PSLAM_OK; }
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
-    uint8_t *dq = nullptr, *dt = nullptr;
-    int32_t *dn = nullptr, *di = nullptr, *dd = nullptr, *dg = nullptr;
     const int capt = nt > 0 ? nt : 1;
     cudaStream_t st = c->stream;
-    int rc = PSLAM_OK;
-#define TRY(call) if (rc == PSLAM_OK) rc = check_cuda(c, (call), #call)
-    TRY(cudaMalloc((void**)&dq, (size_t)nq * 32)); TRY(cudaMalloc((void**)&dt, (size_t)capt * 32)); TRY(cudaMalloc((void**)&dn, 4 * sizeof(int32_t)));
-    TRY(cudaMalloc((void**)&di, (size_t)nq * 2 * sizeof(int32_t))); TRY(cudaMalloc((void**)&dd, (size_t)nq * 2 * sizeof(int32_t)));
-    TRY(cudaMalloc((void**)&dg, (size_t)nq * sizeof(int32_t)));
-    const int32_t counts[4] = {nq, nt, 0, 0};
-    TRY(cudaMemcpyAsync(dq, q, (size_t)nq * 32, cudaMemcpyHostToDevice, st));
-    if (nt) TRY(cudaMemcpyAsync(dt, t, (size_t)nt * 32, cudaMemcpyHostToDevice, st));
-    TRY(cudaMemcpyAsync(dn, counts, sizeof counts, cudaMemcpyHostToDevice, st));
-    if (rc == PSLAM_OK) rc = pslam_hamming_knn2_batch_dev(c, dq, dn, nq, dt, dn + 1, capt, 1, di, dd, good ? dg : nullptr, good ? dn + 2 : nullptr);
-    TRY(cudaMemcpyAsync(idx2, di, (size_t)nq * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    TRY(cudaMemcpyAsync(dist2, dd, (size_t)nq * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    Slab s;
+    const auto dq = s.add<uint8_t>((size_t)nq * 32), dt = s.add<uint8_t>((size_t)capt * 32);
+    const auto dn = s.add<int32_t>(2), dng = s.add<int32_t>(1), di = s.add<int32_t>((size_t)nq * 2), dd = s.add<int32_t>((size_t)nq * 2), dg = s.add<int32_t>(nq);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    const int32_t counts[2] = {nq, nt};
+    s.up(dq, q, st);
+    if (nt) s.up(dt, t, st);
+    s.up(dn, counts, st); s.zero(dng, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    rc = pslam_hamming_knn2_batch_dev(c, s[dq], s[dn], nq, s[dt], s[dn] + 1, capt, 1, s[di], s[dd], good ? s[dg] : nullptr, good ? s[dng] : nullptr);
+    if (rc != PSLAM_OK) return rc;
+    s.down(idx2, di, st); s.down(dist2, dd, st);
     int32_t ng = 0;
-    if (good) { TRY(cudaMemcpyAsync(good, dg, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, st)); TRY(cudaMemcpyAsync(&ng, dn + 2, sizeof ng, cudaMemcpyDeviceToHost, st)); }
-    TRY(cudaStreamSynchronize(st));
-#undef TRY
+    if (good) { s.down(good, dg, st); s.down(&ng, dng, st); }
+    if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
     if (n_good) *n_good = ng;
-    cudaFree(dq); cudaFree(dt); cudaFree(dn); cudaFree(di); cudaFree(dd); cudaFree(dg);
-    return rc;
+    return PSLAM_OK;
 }
 
 }  // extern "C"

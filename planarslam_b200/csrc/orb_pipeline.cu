@@ -87,37 +87,22 @@ int orb_build_geometry(pslam_ctx* c) {
     return PSLAM_OK;
 }
 
-template <typename T>
-static int dmalloc(pslam_ctx* c, T** p, size_t n) { return check_cuda(c, cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)), "cudaMalloc"); }
-
 int orb_alloc(pslam_ctx* c) {
     const OrbGeom& g = c->geom;
     const size_t B = c->cfg.max_batch;
     const int cap = g.total_kp;
     int rc;
-#define A(call) if ((rc = (call)) != PSLAM_OK) return rc
-    A(dmalloc(c, &c->d_gray, B * g.width * g.height));
-    A(dmalloc(c, &c->d_pyr, B * g.pyr_bytes));
-    A(dmalloc(c, &c->d_blur, B * c->blur_frame_bytes));
-    A(dmalloc(c, &c->d_xofs, (size_t)g.total_tabx)); A(dmalloc(c, &c->d_xa, (size_t)2 * g.total_tabx));
-    A(dmalloc(c, &c->d_yofs, (size_t)g.total_taby)); A(dmalloc(c, &c->d_ya, (size_t)2 * g.total_taby));
-    A(dmalloc(c, &c->d_slots, B * g.total_slots));
-    A(dmalloc(c, &c->d_cell_cnt, B * g.total_cells));
-    A(dmalloc(c, &c->d_cand, B * g.total_cand * 2));
-    A(dmalloc(c, &c->d_cand_cnt, B * g.nlevels));
-    A(dmalloc(c, &c->d_nodes, B * g.total_nodes));
-    A(dmalloc(c, &c->d_links, B * g.total_nodes));
-    A(dmalloc(c, &c->d_work, B * g.total_work));
-    A(dmalloc(c, &c->d_lvl_kp, B * g.total_kp));
-    A(dmalloc(c, &c->d_lvl_cnt, B * g.nlevels));
-    A(dmalloc(c, &c->d_kps, B * cap));
-    A(dmalloc(c, &c->d_desc, B * cap * 32));
-    A(dmalloc(c, &c->d_n, B));
-    A(check_cuda(c, cudaMallocHost((void**)&c->h_gray, B * g.width * g.height), "cudaMallocHost"));
-    A(check_cuda(c, cudaMallocHost((void**)&c->h_kps, B * cap * sizeof(pslam_keypoint)), "cudaMallocHost"));
-    A(check_cuda(c, cudaMallocHost((void**)&c->h_desc, B * cap * 32), "cudaMallocHost"));
-    A(check_cuda(c, cudaMallocHost((void**)&c->h_n, B * sizeof(int32_t)), "cudaMallocHost"));
-#undef A
+    if ((rc = c->d_gray.reserve(c, B * g.width * g.height)) || (rc = c->d_pyr.reserve(c, B * g.pyr_bytes)) || (rc = c->d_blur.reserve(c, B * c->blur_frame_bytes)) ||
+        (rc = c->d_xofs.reserve(c, g.total_tabx)) || (rc = c->d_xa.reserve(c, (size_t)2 * g.total_tabx)) ||
+        (rc = c->d_yofs.reserve(c, g.total_taby)) || (rc = c->d_ya.reserve(c, (size_t)2 * g.total_taby)) ||
+        (rc = c->d_slots.reserve(c, B * g.total_slots)) || (rc = c->d_cell_cnt.reserve(c, B * g.total_cells)) ||
+        (rc = c->d_cand.reserve(c, B * g.total_cand * 2)) || (rc = c->d_cand_cnt.reserve(c, B * g.nlevels)) ||
+        (rc = c->d_nodes.reserve(c, B * g.total_nodes)) || (rc = c->d_links.reserve(c, B * g.total_nodes)) || (rc = c->d_work.reserve(c, B * g.total_work)) ||
+        (rc = c->d_lvl_kp.reserve(c, B * g.total_kp)) || (rc = c->d_lvl_cnt.reserve(c, B * g.nlevels)) ||
+        (rc = c->d_kps.reserve(c, B * cap)) || (rc = c->d_desc.reserve(c, B * cap * 32)) || (rc = c->d_n.reserve(c, B)) ||
+        (rc = c->h_gray.reserve(c, B * g.width * g.height)) || (rc = c->h_kps.reserve(c, B * cap)) || (rc = c->h_desc.reserve(c, B * cap * 32)) ||
+        (rc = c->h_n.reserve(c, B)))
+        return rc;
     // resize tables (cv::resize INTER_LINEAR 8-bit: 11-bit coefficients, see oracle/cvprims.cc for the pinned restatement)
     std::vector<int16_t> xofs(g.total_tabx), xa(2 * g.total_tabx), yofs(g.total_taby), ya(2 * g.total_taby);
     for (int l = 1; l < g.nlevels; ++l) {
@@ -148,14 +133,6 @@ int orb_alloc(pslam_ctx* c) {
     PSLAM_CUDA(c, cudaMemcpy(c->d_ya, ya.data(), ya.size() * 2, cudaMemcpyHostToDevice));
     c->orb_ready = true;
     return PSLAM_OK;
-}
-
-void orb_free(pslam_ctx* c) {
-    cudaFree(c->d_gray); cudaFree(c->d_pyr); cudaFree(c->d_blur); cudaFree(c->d_blur_maps); c->d_blur_maps = nullptr; cudaFree(c->d_xofs); cudaFree(c->d_xa); cudaFree(c->d_yofs);
-    cudaFree(c->d_ya); cudaFree(c->d_slots); cudaFree(c->d_cell_cnt); cudaFree(c->d_cand); cudaFree(c->d_cand_cnt);
-    cudaFree(c->d_nodes); cudaFree(c->d_links); cudaFree(c->d_work); cudaFree(c->d_lvl_kp); cudaFree(c->d_lvl_cnt);
-    cudaFree(c->d_kps); cudaFree(c->d_desc); cudaFree(c->d_n);
-    cudaFreeHost(c->h_gray); cudaFreeHost(c->h_kps); cudaFreeHost(c->h_desc); cudaFreeHost(c->h_n);
 }
 
 int orb_run_dev(pslam_ctx* c, const uint8_t* d_gray, int nframes, pslam_keypoint* d_kps, uint8_t* d_desc, int cap, int32_t* d_n) {
@@ -205,7 +182,7 @@ int orb_run_dev(pslam_ctx* c, const uint8_t* d_gray, int nframes, pslam_keypoint
             P.tile_base[g.nlevels] = base; P.nlevels = g.nlevels;
             c->blur_tma_src = tma_ok ? d_gray : nullptr; c->blur_tma_n = nframes;
             if (tma_ok) {
-                if (!c->d_blur_maps) PSLAM_CUDA(c, cudaMalloc((void**)&c->d_blur_maps, sizeof P.map));
+                if (const int rc = c->d_blur_maps.reserve(c, PSLAM_MAX_LEVELS)) return rc;
                 PSLAM_CUDA(c, cudaMemcpyAsync(c->d_blur_maps, P.map, sizeof P.map, cudaMemcpyHostToDevice, st));      // P.map lives in the context: stable until the next re-encode
             }
         }

@@ -39,40 +39,29 @@ int peac_build_geometry(pslam_ctx* c) {
     return PSLAM_OK;
 }
 
-template <typename T>
-static int dmalloc(pslam_ctx* c, T** p, size_t n) { return check_cuda(c, cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)), "cudaMalloc"); }
-
 int peac_alloc(pslam_ctx* c) {
     const PeacGeom& g = c->pgeom;
     const size_t B = c->cfg.max_batch, nb = g.nblk, px = (size_t)g.w * g.h;
     int rc;
-#define A(call) if ((rc = (call)) != PSLAM_OK) return rc
-    A(dmalloc(c, &c->d_depth, B * px));
-    A(dmalloc(c, &c->d_blk_st, B * nb * 9)); A(dmalloc(c, &c->d_blk_geo, B * nb * 8)); A(dmalloc(c, &c->d_blk_n, B * nb)); A(dmalloc(c, &c->d_blk_valid, B * nb));
-    A(dmalloc(c, &c->d_node_st, B * nb * 9)); A(dmalloc(c, &c->d_node_geo, B * nb * 8)); A(dmalloc(c, &c->d_node_n, B * nb));
-    A(dmalloc(c, &c->d_node_rid, B * nb)); A(dmalloc(c, &c->d_node_cid, B * nb)); A(dmalloc(c, &c->d_node_alive, B * nb));
-    A(dmalloc(c, &c->d_adj, B * nb * g.adj_words)); A(dmalloc(c, &c->d_wlo, B * nb)); A(dmalloc(c, &c->d_whi, B * nb)); A(dmalloc(c, &c->d_nb_list, B * nb)); A(dmalloc(c, &c->d_keyf, B * nb));
-    A(dmalloc(c, &c->d_ds_parent, B * nb)); A(dmalloc(c, &c->d_ds_size, B * nb));
-    A(dmalloc(c, &c->d_coarse, B * PEAC_MAX_PLANES)); A(dmalloc(c, &c->d_ncoarse, B)); A(dmalloc(c, &c->d_next_cid, B)); A(dmalloc(c, &c->d_blk_map, B * nb));
-    A(dmalloc(c, &c->d_dist, B * px)); A(dmalloc(c, &c->d_queue, B * g.queue_cap)); A(dmalloc(c, &c->d_qlen, B));
-    A(dmalloc(c, &c->d_pl_adj, B * PEAC_MAX_PLANES * PEAC_PL_WORDS));
-    A(dmalloc(c, &c->d_final, B * PEAC_MAX_PLANES)); A(dmalloc(c, &c->d_scratch, B * (size_t)peac_num_sub(g) * PEAC_MAX_PLANES));
-    A(dmalloc(c, &c->d_final_map, B * PEAC_MAX_PLANES));
-    A(dmalloc(c, &c->d_labels, B * px)); A(dmalloc(c, &c->d_planes, B * PEAC_MAX_PLANES)); A(dmalloc(c, &c->d_nplanes, B));
-    A(dmalloc(c, &c->d_midx, B * px)); A(dmalloc(c, &c->d_moff, B * (PEAC_MAX_PLANES + 1)));
-    A(check_cuda(c, cudaMallocHost((void**)&c->h_depth, B * px * sizeof(uint16_t)), "cudaMallocHost"));
-#undef A
+    if ((rc = c->d_depth.reserve(c, B * px)) ||
+        (rc = c->d_blk_st.reserve(c, B * nb * 9)) || (rc = c->d_blk_geo.reserve(c, B * nb * 8)) || (rc = c->d_blk_n.reserve(c, B * nb)) || (rc = c->d_blk_valid.reserve(c, B * nb)) ||
+        (rc = c->d_node_st.reserve(c, B * nb * 9)) || (rc = c->d_node_geo.reserve(c, B * nb * 8)) || (rc = c->d_node_n.reserve(c, B * nb)) ||
+        (rc = c->d_node_rid.reserve(c, B * nb)) || (rc = c->d_node_cid.reserve(c, B * nb)) || (rc = c->d_node_alive.reserve(c, B * nb)) ||
+        (rc = c->d_adj.reserve(c, B * nb * g.adj_words)) || (rc = c->d_wlo.reserve(c, B * nb)) || (rc = c->d_whi.reserve(c, B * nb)) ||
+        (rc = c->d_nb_list.reserve(c, B * nb)) || (rc = c->d_keyf.reserve(c, B * nb)) ||
+        (rc = c->d_ds_parent.reserve(c, B * nb)) || (rc = c->d_ds_size.reserve(c, B * nb)) ||
+        (rc = c->d_coarse.reserve(c, B * PEAC_MAX_PLANES)) || (rc = c->d_ncoarse.reserve(c, B)) || (rc = c->d_next_cid.reserve(c, B)) ||
+        (rc = c->d_blk_map.reserve(c, B * nb)) ||
+        (rc = c->d_dist.reserve(c, B * px)) || (rc = c->d_queue.reserve(c, B * g.queue_cap)) || (rc = c->d_qlen.reserve(c, B)) ||
+        (rc = c->d_pl_adj.reserve(c, B * PEAC_MAX_PLANES * PEAC_PL_WORDS)) ||
+        (rc = c->d_final.reserve(c, B * PEAC_MAX_PLANES)) || (rc = c->d_scratch.reserve(c, B * (size_t)peac_num_sub(g) * PEAC_MAX_PLANES)) ||
+        (rc = c->d_final_map.reserve(c, B * PEAC_MAX_PLANES)) ||
+        (rc = c->d_labels.reserve(c, B * px)) || (rc = c->d_planes.reserve(c, B * PEAC_MAX_PLANES)) || (rc = c->d_nplanes.reserve(c, B)) ||
+        (rc = c->d_midx.reserve(c, B * px)) || (rc = c->d_moff.reserve(c, B * (PEAC_MAX_PLANES + 1))) ||
+        (rc = c->h_depth.reserve(c, B * px)))
+        return rc;
     c->peac_ready = true;
     return PSLAM_OK;
-}
-
-void peac_free(pslam_ctx* c) {
-    cudaFree(c->d_depth); cudaFree(c->d_blk_st); cudaFree(c->d_blk_geo); cudaFree(c->d_blk_n); cudaFree(c->d_blk_valid);
-    cudaFree(c->d_node_st); cudaFree(c->d_node_geo); cudaFree(c->d_node_n); cudaFree(c->d_node_rid); cudaFree(c->d_node_cid);
-    cudaFree(c->d_node_alive); cudaFree(c->d_adj); cudaFree(c->d_wlo); cudaFree(c->d_whi); cudaFree(c->d_nb_list); cudaFree(c->d_keyf); cudaFree(c->d_ds_parent); cudaFree(c->d_ds_size);
-    cudaFree(c->d_coarse); cudaFree(c->d_ncoarse); cudaFree(c->d_next_cid); cudaFree(c->d_blk_map); cudaFree(c->d_dist); cudaFree(c->d_queue);
-    cudaFree(c->d_qlen); cudaFree(c->d_pl_adj); cudaFree(c->d_final); cudaFree(c->d_scratch); cudaFree(c->d_final_map); cudaFree(c->d_labels); cudaFree(c->d_planes);
-    cudaFree(c->d_nplanes); cudaFree(c->d_midx); cudaFree(c->d_moff); cudaFreeHost(c->h_depth);
 }
 
 // resident-CTA target of the clustering kernel (see k_peac_cluster): PSLAM_PEAC_OCC = 12 (default), 16 or 20

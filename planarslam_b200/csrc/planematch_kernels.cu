@@ -68,36 +68,25 @@ extern "C" int pslam_plane_match(pslam_ctx* c, const float* Tcw, int n_frame, co
             pM[4 * i + r] = (float)s;
         }
     const int npts = pts_off[n_map];
-    const size_t bytes = 256 * 12 + pM.size() * 4 + (size_t)n_map * 4 * 4 + n_map + (size_t)(n_map + 1) * 4 + (size_t)npts * 12 +
-                         (size_t)n_frame * n_map * 8 + (size_t)n_frame * 12 + 16;
-    uint8_t* blob = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&blob, bytes));
-    uint8_t* p = blob;
-    auto carve = [&](size_t n) { uint8_t* r = p; p += (n + 255) / 256 * 256; return r; };
-    float* d_pM = (float*)carve(pM.size() * 4); float* d_mc = (float*)carve((size_t)n_map * 16); uint8_t* d_bad = carve(n_map);
-    int32_t* d_off = (int32_t*)carve((size_t)(n_map + 1) * 4); float* d_pts = (float*)carve((size_t)npts * 12 + 4);
-    float* d_ang = (float*)carve((size_t)n_frame * n_map * 4); float* d_min = (float*)carve((size_t)n_frame * n_map * 4);
-    int32_t* d_out = (int32_t*)carve((size_t)n_frame * 12 + 16);
-    cudaStream_t st = c->stream;
-    int rc = PSLAM_OK;
-#define TRY(call) if (rc == PSLAM_OK) rc = check_cuda(c, (call), #call)
-    TRY(cudaMemcpyAsync(d_pM, pM.data(), pM.size() * 4, cudaMemcpyHostToDevice, st));
-    TRY(cudaMemcpyAsync(d_mc, map_coef, (size_t)n_map * 16, cudaMemcpyHostToDevice, st));
-    TRY(cudaMemcpyAsync(d_bad, map_bad, n_map, cudaMemcpyHostToDevice, st));
-    TRY(cudaMemcpyAsync(d_off, pts_off, (size_t)(n_map + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (npts) TRY(cudaMemcpyAsync(d_pts, pts, (size_t)npts * 12, cudaMemcpyHostToDevice, st));
-    TRY(cudaMemsetAsync(d_out + 3 * n_frame, 0, sizeof(int32_t), st));
-    if (rc == PSLAM_OK) {
-        PSLAM_LAUNCH(c, "plane_pairs", k_plane_pairs<<<(n_frame * n_map + 7) / 8, 256, 0, st>>>(n_frame, n_map, d_pM, d_mc, d_off, d_pts, d_ang, d_min));
-        PSLAM_LAUNCH(c, "plane_assign", k_plane_assign<<<(n_frame + 63) / 64, 64, 0, st>>>(n_frame, n_map, d_bad, d_ang, d_min, dTh, aTh, verTh, parTh, d_out,
-                     d_out + n_frame, d_out + 2 * n_frame, d_out + 3 * n_frame));
-    }
-    std::vector<int32_t> out((size_t)3 * n_frame + 1);
-    TRY(cudaMemcpyAsync(out.data(), d_out, out.size() * 4, cudaMemcpyDeviceToHost, st));
-    TRY(cudaStreamSynchronize(st));
-#undef TRY
-    cudaFree(blob);
+    Slab s;
+    const auto d_pM = s.add<float>(pM.size()), d_mc = s.add<float>((size_t)n_map * 4);
+    const auto d_bad = s.add<uint8_t>(n_map);
+    const auto d_off = s.add<int32_t>(n_map + 1);
+    const auto d_pts = s.add<float>((size_t)npts * 3 + 1), d_ang = s.add<float>((size_t)n_frame * n_map), d_min = s.add<float>((size_t)n_frame * n_map);
+    const auto d_out = s.add<int32_t>((size_t)n_frame * 3), d_cnt = s.add<int32_t>(1);      // match, ver, par; number of matches
+    int rc = s.alloc(c);
     if (rc != PSLAM_OK) return rc;
+    cudaStream_t st = c->stream;
+    s.up(d_pM, pM.data(), st); s.up(d_mc, map_coef, st); s.up(d_bad, map_bad, st); s.up(d_off, pts_off, st); s.up(d_pts, pts, st, (size_t)npts * 3);
+    s.zero(d_cnt, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    int32_t* out_d = s[d_out];
+    PSLAM_LAUNCH(c, "plane_pairs", k_plane_pairs<<<(n_frame * n_map + 7) / 8, 256, 0, st>>>(n_frame, n_map, s[d_pM], s[d_mc], s[d_off], s[d_pts], s[d_ang], s[d_min]));
+    PSLAM_LAUNCH(c, "plane_assign", k_plane_assign<<<(n_frame + 63) / 64, 64, 0, st>>>(n_frame, n_map, s[d_bad], s[d_ang], s[d_min], dTh, aTh, verTh, parTh, out_d,
+                 out_d + n_frame, out_d + 2 * n_frame, s[d_cnt]));
+    std::vector<int32_t> out((size_t)3 * n_frame + 1);
+    s.down(out.data(), d_out, st); s.down(out.data() + 3 * n_frame, d_cnt, st);
+    if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
     for (int i = 0; i < n_frame; ++i) { match[i] = out[i]; ver[i] = out[n_frame + i]; par[i] = out[2 * n_frame + i]; }
     return out[3 * n_frame];
 }

@@ -31,10 +31,10 @@ namespace pslam {
 struct PlanePostBuffers {
     int max_batch = 0, maxp = 0, w3 = 0, h3 = 0;
     // per (frame, plane) working records
-    float* d_coef = nullptr; int32_t* d_valid = nullptr; int32_t* d_npts = nullptr; float* d_pts = nullptr; int32_t* d_stats = nullptr;     // [B][maxp][...]
+    DevArray<float> d_coef; DevArray<int32_t> d_valid, d_npts; DevArray<float> d_pts; DevArray<int32_t> d_stats;     // [B][maxp][...]
     // surface normals scratch
-    float* d_cloud = nullptr; float* d_dist = nullptr; double *d_ix = nullptr, *d_iy = nullptr;
-    float* d_nrm = nullptr;
+    DevArray<float> d_cloud, d_dist; DevArray<double> d_ix, d_iy;
+    DevArray<float> d_nrm;
 };
 
 struct PPCam { float fx, fy, cx, cy, scale; };
@@ -573,10 +573,6 @@ __global__ void k_sn_gather(int W3, int H3, const float* __restrict__ cloud_all,
 }
 
 void planepost_free(pslam_ctx* c) {
-    if (!c->planepost) return;
-    PlanePostBuffers& B = *c->planepost;
-    for (void* p : {(void*)B.d_coef, (void*)B.d_valid, (void*)B.d_npts, (void*)B.d_pts, (void*)B.d_stats, (void*)B.d_cloud, (void*)B.d_dist, (void*)B.d_ix, (void*)B.d_iy, (void*)B.d_nrm})
-        if (p) cudaFree(p);
     delete c->planepost;
     c->planepost = nullptr;
 }
@@ -601,12 +597,14 @@ static int planepost_alloc(pslam_ctx* c) {
         if (rc_ != PSLAM_OK) { planepost_free(c); return rc_; }
     }
     const size_t nb = B.max_batch, np = (size_t)B.w3 * B.h3, ni = (size_t)(B.w3 + 1) * (B.h3 + 1);
-#define PA(ptr, bytes) do { const int rc_ = check_cuda(c, cudaMalloc((void**)&(ptr), (bytes)), "cudaMalloc(planepost)"); if (rc_ != PSLAM_OK) { planepost_free(c); return rc_; } } while (0)
-    PA(B.d_coef, nb * B.maxp * 16); PA(B.d_valid, nb * B.maxp * 4); PA(B.d_npts, nb * B.maxp * 4); PA(B.d_stats, nb * B.maxp * 8);
-    PA(B.d_pts, nb * B.maxp * (size_t)PP_SLOTS * 12);
-    PA(B.d_cloud, nb * np * 12); PA(B.d_dist, nb * (np + 2) * 4);
-    PA(B.d_ix, nb * ni * 24); PA(B.d_iy, nb * ni * 24); PA(B.d_nrm, nb * np * 12);
-#undef PA
+    int rc;
+    if ((rc = B.d_coef.reserve(c, nb * B.maxp * 4)) || (rc = B.d_valid.reserve(c, nb * B.maxp)) || (rc = B.d_npts.reserve(c, nb * B.maxp)) ||
+        (rc = B.d_stats.reserve(c, nb * B.maxp * 2)) || (rc = B.d_pts.reserve(c, nb * B.maxp * (size_t)PP_SLOTS * 3)) ||
+        (rc = B.d_cloud.reserve(c, nb * np * 3)) || (rc = B.d_dist.reserve(c, nb * (np + 2))) ||
+        (rc = B.d_ix.reserve(c, nb * ni * 3)) || (rc = B.d_iy.reserve(c, nb * ni * 3)) || (rc = B.d_nrm.reserve(c, nb * np * 3))) {
+        planepost_free(c);
+        return rc;
+    }
     return PSLAM_OK;
 }
 
@@ -679,30 +677,32 @@ int pslam_compute_planes_batch(pslam_ctx* c, const uint16_t* depth, int nframes,
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     const int maxp = pslam_peac_max_planes(c), n_sn = pslam_surface_normals_count(c);
     const size_t npx = (size_t)c->cfg.width * c->cfg.height, nf = (size_t)nframes;
-    const size_t sz[] = {nf * npx * 2, nf * npx * 4, nf * maxp * sizeof(pslam_plane), nf * 4, nf * npx * 4, nf * (maxp + 1) * 4, nf * 4, nf * maxp * 4, nf * maxp * 16,
-                         nf * (maxp + 1) * 4, nf * cap_pts * 12, nf * 4, nf * n_sn * 32};
-    size_t off[14]; off[0] = 0;
-    for (int i = 0; i < 13; ++i) off[i + 1] = (off[i] + sz[i] + 255) & ~(size_t)255;
-    uint8_t* d = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&d, off[13]));
+    Slab s;
+    const auto d_depth = s.add<uint16_t>(nf * npx);
+    const auto labels = s.add<int32_t>(nf * npx);
+    const auto planes = s.add<pslam_plane>(nf * maxp);
+    const auto nplanes = s.add<int32_t>(nf), members = s.add<int32_t>(nf * npx), moff = s.add<int32_t>(nf * (maxp + 1));
+    const auto d_kept = s.add<int32_t>(nf), d_src = s.add<int32_t>(nf * maxp);
+    const auto d_coef = s.add<float>(nf * maxp * 4);
+    const auto d_off = s.add<int32_t>(nf * (maxp + 1));
+    const auto d_pts = s.add<float>(nf * cap_pts * 3);
+    const auto d_status = s.add<int32_t>(nf);
+    const auto d_normals8 = s.add<float>(nf * n_sn * 8);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
     cudaStream_t st = c->stream;
-    cudaMemcpyAsync(d + off[0], depth, sz[0], cudaMemcpyHostToDevice, st);
-    int rc = pslam_peac_run_batch_dev(c, (const uint16_t*)(d + off[0]), nframes, (int32_t*)(d + off[1]), (pslam_plane*)(d + off[2]), (int32_t*)(d + off[3]), (int32_t*)(d + off[4]),
-                                      (int32_t*)(d + off[5]));
+    s.up(d_depth, depth, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    rc = pslam_peac_run_batch_dev(c, s[d_depth], nframes, s[labels], s[planes], s[nplanes], s[members], s[moff]);
     if (rc == PSLAM_OK)
-        rc = pslam_planes_post_batch_dev(c, (const uint16_t*)(d + off[0]), nframes, (const pslam_plane*)(d + off[2]), (const int32_t*)(d + off[3]), (const int32_t*)(d + off[4]),
-                                         (const int32_t*)(d + off[5]), dist_th, (int32_t*)(d + off[6]), (int32_t*)(d + off[7]), (float*)(d + off[8]), (int32_t*)(d + off[9]),
-                                         (float*)(d + off[10]), cap_pts, (int32_t*)(d + off[11]));
-    if (rc == PSLAM_OK && normals8) rc = pslam_surface_normals_batch_dev(c, (const uint16_t*)(d + off[0]), nframes, (float*)(d + off[12]), nullptr);
-    if (rc != PSLAM_OK) { cudaStreamSynchronize(st); cudaFree(d); return rc; }
+        rc = pslam_planes_post_batch_dev(c, s[d_depth], nframes, s[planes], s[nplanes], s[members], s[moff], dist_th, s[d_kept], s[d_src], s[d_coef], s[d_off], s[d_pts],
+                                         cap_pts, s[d_status]);
+    if (rc == PSLAM_OK && normals8) rc = pslam_surface_normals_batch_dev(c, s[d_depth], nframes, s[d_normals8], nullptr);
+    if (rc != PSLAM_OK) { cudaStreamSynchronize(st); return rc; }
     std::vector<int32_t> status(nframes);
-    cudaMemcpyAsync(n_kept, d + off[6], sz[6], cudaMemcpyDeviceToHost, st); cudaMemcpyAsync(src, d + off[7], sz[7], cudaMemcpyDeviceToHost, st);
-    cudaMemcpyAsync(coef, d + off[8], sz[8], cudaMemcpyDeviceToHost, st); cudaMemcpyAsync(pt_off, d + off[9], sz[9], cudaMemcpyDeviceToHost, st);
-    cudaMemcpyAsync(pts, d + off[10], sz[10], cudaMemcpyDeviceToHost, st); cudaMemcpyAsync(status.data(), d + off[11], sz[11], cudaMemcpyDeviceToHost, st);
-    if (normals8) cudaMemcpyAsync(normals8, d + off[12], sz[12], cudaMemcpyDeviceToHost, st);
-    const cudaError_t e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    if (e != cudaSuccess) return check_cuda(c, e, "compute planes");
+    s.down(n_kept, d_kept, st); s.down(src, d_src, st); s.down(coef, d_coef, st); s.down(pt_off, d_off, st); s.down(pts, d_pts, st); s.down(status.data(), d_status, st);
+    if (normals8) s.down(normals8, d_normals8, st);
+    if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;
     for (int f = 0; f < nframes; ++f) if (status[f] & (32 | 64)) return set_error(c, PSLAM_E_CAPACITY, "more voxels than the plane post-processing capacity");
     return PSLAM_OK;
 }

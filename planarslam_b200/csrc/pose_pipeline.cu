@@ -14,11 +14,10 @@ struct PoseBuffers {
     std::vector<float4> h_pa, h_pb;          // point records (one slot per edge; line / plane slots stay zero)
     std::vector<PoseEdgeDev> h_wide;         // line and plane records
     // device
-    PoseHeaderDev* d_hdr = nullptr; float4* d_pa = nullptr; float4* d_pb = nullptr; PoseEdgeDev* d_wide = nullptr; double* d_pjac = nullptr;
-    uint8_t* d_level = nullptr;
-    uint8_t* d_flags[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    PoseOutDev* d_out = nullptr;
-    size_t cap_prob = 0, cap_out = 0, cap_pa = 0, cap_pb = 0, cap_wide = 0, cap_pjac = 0, cap_level = 0, cap_flags[5] = {0, 0, 0, 0, 0};   // one capacity per buffer (elements)
+    DevArray<PoseHeaderDev> d_hdr; DevArray<float4> d_pa, d_pb; DevArray<PoseEdgeDev> d_wide; DevArray<double> d_pjac;
+    DevArray<uint8_t> d_level;
+    DevArray<uint8_t> d_flags[5];
+    DevArray<PoseOutDev> d_out;
     int n_prob = 0;
     int tot_flags[5] = {0, 0, 0, 0, 0};
     std::vector<PoseOutDev> h_out;
@@ -33,17 +32,6 @@ static void plane_from_float4(const float* v, double out[4]) {     // Converter:
     for (int i = 0; i < 4; ++i) p[i] = p[i] * s;
     if (p[3] < 0.0) for (int i = 0; i < 4; ++i) p[i] = -p[i];
     for (int i = 0; i < 4; ++i) out[i] = p[i];
-}
-
-template <typename T>
-static int grow(pslam_ctx* c, T** p, size_t* cap, size_t need) {
-    if (need <= *cap) return PSLAM_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    const size_t n = std::max<size_t>(need * 3 / 2, 64);
-    int rc = check_cuda(c, cudaMalloc((void**)p, n * sizeof(T)), "cudaMalloc(pose)");
-    *cap = rc == PSLAM_OK ? n : 0;
-    return rc;
 }
 
 int pose_pack_upload(pslam_ctx* c, const pslam_pose_problem* probs, int n, const float* Tcw0, int mode) {
@@ -127,14 +115,10 @@ int pose_pack_upload(pslam_ctx* c, const pslam_pose_problem* probs, int n, const
     for (int k = 0; k < 5; ++k) B.tot_flags[k] = off[k];
     const size_t n_edges = B.h_pa.size();
     int rc;
-    if ((rc = grow(c, &B.d_hdr, &B.cap_prob, (size_t)n)) != PSLAM_OK) return rc;
-    if ((rc = grow(c, &B.d_out, &B.cap_out, (size_t)n)) != PSLAM_OK) return rc;
-    if ((rc = grow(c, &B.d_pa, &B.cap_pa, n_edges)) != PSLAM_OK) return rc;
-    if ((rc = grow(c, &B.d_pb, &B.cap_pb, n_edges)) != PSLAM_OK) return rc;
-    if ((rc = grow(c, &B.d_wide, &B.cap_wide, B.h_wide.size())) != PSLAM_OK) return rc;
-    if ((rc = grow(c, &B.d_pjac, &B.cap_pjac, (size_t)n_plane_edges * 36)) != PSLAM_OK) return rc;
-    if ((rc = grow(c, &B.d_level, &B.cap_level, n_edges)) != PSLAM_OK) return rc;
-    for (int k = 0; k < 5; ++k) if ((rc = grow(c, &B.d_flags[k], &B.cap_flags[k], (size_t)std::max(off[k], 1))) != PSLAM_OK) return rc;
+    if ((rc = B.d_hdr.grow(c, n)) || (rc = B.d_out.grow(c, n)) || (rc = B.d_pa.grow(c, n_edges)) || (rc = B.d_pb.grow(c, n_edges)) ||
+        (rc = B.d_wide.grow(c, B.h_wide.size())) || (rc = B.d_pjac.grow(c, (size_t)n_plane_edges * 36)) || (rc = B.d_level.grow(c, n_edges)))
+        return rc;
+    for (int k = 0; k < 5; ++k) if ((rc = B.d_flags[k].grow(c, std::max(off[k], 1)))) return rc;
     cudaStream_t st = c->stream;
     PSLAM_CUDA(c, cudaMemcpyAsync(B.d_hdr, B.h_hdr.data(), n * sizeof(PoseHeaderDev), cudaMemcpyHostToDevice, st));
     PSLAM_CUDA(c, cudaMemcpyAsync(B.d_pa, B.h_pa.data(), n_edges * sizeof(float4), cudaMemcpyHostToDevice, st));
@@ -178,10 +162,6 @@ int pose_fetch(pslam_ctx* c, float* Tcw, double* Tcw_d, uint8_t* o_pt, uint8_t* 
 }
 
 void pose_free(pslam_ctx* c) {
-    if (!c->pose) return;
-    PoseBuffers& B = *c->pose;
-    cudaFree(B.d_hdr); cudaFree(B.d_pa); cudaFree(B.d_pb); cudaFree(B.d_wide); cudaFree(B.d_pjac); cudaFree(B.d_level); cudaFree(B.d_out);
-    for (int k = 0; k < 5; ++k) cudaFree(B.d_flags[k]);
     delete c->pose;
     c->pose = nullptr;
 }

@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "../../include/pslam_abi.h"
+#include "devmem.h"
 
 #define PSLAM_MAX_LEVELS 8
 
@@ -105,41 +106,41 @@ struct pslam_ctx {
     bool orb_ready = false, peac_ready = false;   // stage buffers are allocated on first use of the stage
 
     // device buffers (sized for cfg.max_batch frames)
-    uint8_t* d_gray = nullptr;        // staging copy of host input (host-pointer entry points)
-    const uint8_t* d_gray_cur = nullptr;  // input of the most recent call (staging or caller's device buffer)
-    uint8_t* d_pyr = nullptr;         // levels 1.. of every frame
-    uint8_t* d_blur = nullptr;        // blurred levels 0.. of every frame (same layout incl. level 0)
+    pslam::DevArray<uint8_t> d_gray;          // staging copy of host input (host-pointer entry points)
+    const uint8_t* d_gray_cur = nullptr;      // input of the most recent call (staging or caller's device buffer)
+    pslam::DevArray<uint8_t> d_pyr;           // levels 1.. of every frame
+    pslam::DevArray<uint8_t> d_blur;          // blurred levels 0.. of every frame (same layout incl. level 0)
     int blur_frame_bytes = 0;
-    pslam::BlurTmaParams blur_tma;    // tensor maps of the TMA-staged blur (orb_pipeline.cu); valid for (blur_tma_src, blur_tma_n)
+    pslam::BlurTmaParams blur_tma;            // tensor maps of the TMA-staged blur (orb_pipeline.cu); valid for (blur_tma_src, blur_tma_n)
     const uint8_t* blur_tma_src = nullptr; int blur_tma_n = 0;
-    CUtensorMap* d_blur_maps = nullptr;      // device copy of blur_tma.map (what the copy engine reads)
-    int16_t* d_xofs = nullptr; int16_t* d_xa = nullptr;   // resize tables: source column, (alpha0, alpha1) pairs
-    int16_t* d_yofs = nullptr; int16_t* d_ya = nullptr;
-    uint32_t* d_slots = nullptr;      // per-cell candidate slots (packed x | y<<11 | score<<22)
-    int32_t* d_cell_cnt = nullptr;    // per-cell candidate counts
-    uint32_t* d_cand = nullptr;       // ordered candidates per (frame, level), ping-pong x2
-    int32_t* d_cand_cnt = nullptr;    // [frame][level]
-    int4* d_nodes = nullptr;          // quadtree node pool
-    int2* d_links = nullptr;
-    int32_t* d_work = nullptr;        // quadtree scratch (expandable lists, list-order array)
-    uint32_t* d_lvl_kp = nullptr;     // selected keypoints per (frame, level) in list order (packed)
-    int32_t* d_lvl_cnt = nullptr;     // [frame][level]
-    int32_t* d_status = nullptr;      // per-frame capacity flags
-    pslam_keypoint* d_kps = nullptr;  // outputs for host-pointer entry points
-    uint8_t* d_desc = nullptr;
-    int32_t* d_n = nullptr;
+    pslam::DevArray<CUtensorMap> d_blur_maps; // device copy of blur_tma.map (what the copy engine reads)
+    pslam::DevArray<int16_t> d_xofs, d_xa;    // resize tables: source column, (alpha0, alpha1) pairs
+    pslam::DevArray<int16_t> d_yofs, d_ya;
+    pslam::DevArray<uint32_t> d_slots;        // per-cell candidate slots (packed x | y<<11 | score<<22)
+    pslam::DevArray<int32_t> d_cell_cnt;      // per-cell candidate counts
+    pslam::DevArray<uint32_t> d_cand;         // ordered candidates per (frame, level), ping-pong x2
+    pslam::DevArray<int32_t> d_cand_cnt;      // [frame][level]
+    pslam::DevArray<int4> d_nodes;            // quadtree node pool
+    pslam::DevArray<int2> d_links;
+    pslam::DevArray<int32_t> d_work;          // quadtree scratch (expandable lists, list-order array)
+    pslam::DevArray<uint32_t> d_lvl_kp;       // selected keypoints per (frame, level) in list order (packed)
+    pslam::DevArray<int32_t> d_lvl_cnt;       // [frame][level]
+    pslam::DevArray<int32_t> d_status;        // per-frame capacity flags
+    pslam::DevArray<pslam_keypoint> d_kps;    // outputs for host-pointer entry points
+    pslam::DevArray<uint8_t> d_desc;
+    pslam::DevArray<int32_t> d_n;
     // ---- PEAC ----
     pslam::PeacGeom pgeom;
-    uint16_t* d_depth = nullptr;                 // staging copy of host depth
-    double* d_blk_st = nullptr; double* d_blk_geo = nullptr; int32_t* d_blk_n = nullptr; uint8_t* d_blk_valid = nullptr;
-    double* d_node_st = nullptr; double* d_node_geo = nullptr; int32_t* d_node_n = nullptr; int32_t* d_node_rid = nullptr;
-    int32_t* d_node_cid = nullptr; uint8_t* d_node_alive = nullptr; uint32_t* d_adj = nullptr; int16_t* d_wlo = nullptr; int16_t* d_whi = nullptr;
-    int32_t* d_nb_list = nullptr; float* d_keyf = nullptr; int32_t* d_ds_parent = nullptr; int32_t* d_ds_size = nullptr;
-    pslam::PeacPlaneRec* d_coarse = nullptr; int32_t* d_ncoarse = nullptr; int32_t* d_next_cid = nullptr; int32_t* d_blk_map = nullptr;
-    float* d_dist = nullptr; uint32_t* d_queue = nullptr; int32_t* d_qlen = nullptr; uint32_t* d_pl_adj = nullptr;
-    pslam::PeacPlaneRec* d_final = nullptr; int32_t* d_scratch = nullptr; int32_t* d_final_map = nullptr;
-    int32_t* d_labels = nullptr; pslam_plane* d_planes = nullptr; int32_t* d_nplanes = nullptr; int32_t* d_midx = nullptr; int32_t* d_moff = nullptr;
-    uint16_t* h_depth = nullptr;                 // pinned
+    pslam::DevArray<uint16_t> d_depth;        // staging copy of host depth
+    pslam::DevArray<double> d_blk_st, d_blk_geo; pslam::DevArray<int32_t> d_blk_n; pslam::DevArray<uint8_t> d_blk_valid;
+    pslam::DevArray<double> d_node_st, d_node_geo; pslam::DevArray<int32_t> d_node_n, d_node_rid, d_node_cid; pslam::DevArray<uint8_t> d_node_alive;
+    pslam::DevArray<uint32_t> d_adj; pslam::DevArray<int16_t> d_wlo, d_whi;
+    pslam::DevArray<int32_t> d_nb_list; pslam::DevArray<float> d_keyf; pslam::DevArray<int32_t> d_ds_parent, d_ds_size;
+    pslam::DevArray<pslam::PeacPlaneRec> d_coarse; pslam::DevArray<int32_t> d_ncoarse, d_next_cid, d_blk_map;
+    pslam::DevArray<float> d_dist; pslam::DevArray<uint32_t> d_queue; pslam::DevArray<int32_t> d_qlen; pslam::DevArray<uint32_t> d_pl_adj;
+    pslam::DevArray<pslam::PeacPlaneRec> d_final; pslam::DevArray<int32_t> d_scratch, d_final_map;
+    pslam::DevArray<int32_t> d_labels; pslam::DevArray<pslam_plane> d_planes; pslam::DevArray<int32_t> d_nplanes, d_midx, d_moff;
+    pslam::PinnedArray<uint16_t> h_depth;
     pslam::PoseBuffers* pose = nullptr;          // pose-optimisation staging (pose_pipeline.cu)
     pslam::SearchBuffers* search = nullptr;      // projection-search staging (search_kernels.cu)
     pslam::LbaBuffers* lba = nullptr;            // local bundle adjustment staging (lba_pipeline.cu)
@@ -151,8 +152,8 @@ struct pslam_ctx {
     pslam::BowVocBuffers* bowvoc = nullptr;      // resident DBoW2 vocabulary + batched-transform scratch (bow_transform_kernels.cu)
     pslam::ExchangeBuffers* exchange = nullptr;  // key-frame descriptor exchange over peer memory (exchange_kernels.cu)
     // pinned host staging
-    uint8_t* h_gray = nullptr; pslam_keypoint* h_kps = nullptr; uint8_t* h_desc = nullptr; int32_t* h_n = nullptr;
-    int32_t* h_status = nullptr;
+    pslam::PinnedArray<uint8_t> h_gray; pslam::PinnedArray<pslam_keypoint> h_kps; pslam::PinnedArray<uint8_t> h_desc; pslam::PinnedArray<int32_t> h_n;
+    pslam::PinnedArray<int32_t> h_status;
 };
 
 namespace pslam {
@@ -161,7 +162,6 @@ int check_cuda(pslam_ctx* c, cudaError_t e, const char* what);
 // ORB pipeline (orb_pipeline.cu)
 int orb_build_geometry(pslam_ctx* c);
 int orb_alloc(pslam_ctx* c);
-void orb_free(pslam_ctx* c);
 int orb_run_dev(pslam_ctx* c, const uint8_t* d_gray, int nframes, pslam_keypoint* d_kps, uint8_t* d_desc, int cap,
                 int32_t* d_n);
 // pose optimisation (pose_pipeline.cu)
@@ -179,7 +179,6 @@ int lsd_status_fetch_async(pslam_ctx* c, int nframes, int32_t* h_pinned);
 // PEAC pipeline (peac_pipeline.cu)
 int peac_build_geometry(pslam_ctx* c);
 int peac_alloc(pslam_ctx* c);
-void peac_free(pslam_ctx* c);
 int peac_run_dev(pslam_ctx* c, const uint16_t* d_depth, int nframes, int32_t* d_labels, pslam_plane* d_planes, int32_t* d_nplanes,
                  int32_t* d_member_idx, int32_t* d_member_off);
 }  // namespace pslam

@@ -5,60 +5,52 @@ namespace pslam {
 
 // ---------------------------------------------------------------------------------------------------------
 struct SearchBuffers {
-    void* blob = nullptr; size_t cap = 0;
-    uint32_t* d_cand = nullptr; int32_t* d_cand_n = nullptr; size_t cap_pts = 0;
-    int32_t *d_cell_start = nullptr, *d_items = nullptr, *d_matches = nullptr, *d_scalar = nullptr, *d_hist_idx = nullptr;
-    int8_t* d_hist_bin = nullptr; uint8_t* d_in_view = nullptr;
+    DevArray<uint8_t> blob;                                     // the frame / map arrays of the current call
+    DevArray<uint32_t> d_cand; DevArray<int32_t> d_cand_n, d_hist_idx; DevArray<int8_t> d_hist_bin; DevArray<uint8_t> d_in_view;   // per point
+    DevArray<int32_t> d_cell_start, d_items, d_matches, d_scalar;
 };
 
-template <typename T>
-static T* carve(uint8_t*& p, size_t n) { T* r = reinterpret_cast<T*>(p); p += (n * sizeof(T) + 255) / 256 * 256; return r; }
-
 static int ensure(pslam_ctx* c, SearchBuffers& B, size_t npts) {
-    if (!B.d_cell_start) {
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_cell_start, (SG_CELLS + 1) * sizeof(int32_t)));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_items, SEARCH_MAX_KP * sizeof(int32_t)));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_matches, SEARCH_MAX_KP * sizeof(int32_t)));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_scalar, 4 * sizeof(int32_t)));
-    }
-    if (npts > B.cap_pts) {
-        cudaFree(B.d_cand); cudaFree(B.d_cand_n); cudaFree(B.d_hist_idx); cudaFree(B.d_hist_bin); cudaFree(B.d_in_view);
-        const size_t n = npts * 3 / 2 + 64;
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_cand, n * SEARCH_CAND_CAP * sizeof(uint32_t)));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_cand_n, n * sizeof(int32_t)));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_hist_idx, n * sizeof(int32_t)));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_hist_bin, n));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_in_view, n));
-        B.cap_pts = n;
-    }
+    int rc;
+    if ((rc = B.d_cell_start.reserve(c, SG_CELLS + 1)) || (rc = B.d_items.reserve(c, SEARCH_MAX_KP)) || (rc = B.d_matches.reserve(c, SEARCH_MAX_KP)) ||
+        (rc = B.d_scalar.reserve(c, 4)) || (rc = B.d_cand.grow(c, npts * SEARCH_CAND_CAP)) || (rc = B.d_cand_n.grow(c, npts)) ||
+        (rc = B.d_hist_idx.grow(c, npts)) || (rc = B.d_hist_bin.grow(c, npts)) || (rc = B.d_in_view.grow(c, npts)))
+        return rc;
     return PSLAM_OK;
 }
 
-// uploads the frame / map arrays into one staging blob; fills the device views
+// uploads the frame / map arrays into the staging blob; fills the device views.  Every array gets at least one element, so no view is null.
 static int upload(pslam_ctx* c, SearchBuffers& B, const pslam_frame_view* f, const pslam_map_points* m, const pslam_last_frame* l, SearchFrameDev& F,
                   SearchMapDev& M, SearchLastDev& Ld) {
     const size_t nf = f->n, nm = m->n, nl = l ? l->n : 0;
-    const size_t need = 4096 + nf * (28 + 4 + 32) + nm * (12 + 12 + 4 + 4 + 32 + 1 + 1) + nl * (28 + 4 + 1) + 256 * 16;
-    if (need > B.cap) { cudaFree(B.blob); B.blob = nullptr; B.cap = 0; PSLAM_CUDA(c, cudaMalloc(&B.blob, need * 3 / 2)); B.cap = need * 3 / 2; }
-    uint8_t* p = (uint8_t*)B.blob;
+    auto one = [](size_t n) { return std::max<size_t>(n, 1); };
+    Slab s;
+    const auto f_keys = s.add<pslam_keypoint>(one(nf)); const auto f_ur = s.add<float>(one(nf)); const auto f_desc = s.add<uint8_t>(one(nf * 32));
+    const auto m_pos = s.add<float>(one(nm * 3)); const auto m_normal = s.add<float>(one(nm * 3)); const auto m_maxd = s.add<float>(one(nm));
+    const auto m_mind = s.add<float>(one(nm)); const auto m_desc = s.add<uint8_t>(one(nm * 32)); const auto m_skip = s.add<uint8_t>(one(nm));
+    const auto m_has_obs = s.add<uint8_t>(one(nm));
+    const auto l_keys = s.add<pslam_keypoint>(one(nl)); const auto l_mp = s.add<int32_t>(one(nl)); const auto l_outlier = s.add<uint8_t>(one(nl));
+    if (const int rc = s.alloc(c, B.blob, true)) return rc;
     cudaStream_t st = c->stream;
-#define UP(dst, src, type, count) { type* d_ = carve<type>(p, (count) ? (count) : 1); if (count) PSLAM_CUDA(c, cudaMemcpyAsync(d_, src, (size_t)(count) * sizeof(type), cudaMemcpyHostToDevice, st)); dst = d_; }
+    s.up(f_keys, f->keys_un, st, nf); s.up(f_ur, f->u_right, st, nf); s.up(f_desc, f->desc, st, nf * 32);
+    s.up(m_pos, m->pos, st, nm * 3); s.up(m_normal, m->normal, st, nm * 3); s.up(m_maxd, m->max_distance, st, nm); s.up(m_mind, m->min_distance, st, nm);
+    s.up(m_desc, m->desc, st, nm * 32); s.up(m_skip, m->skip, st, nm); s.up(m_has_obs, m->has_obs, st, nm);
+    if (l) { s.up(l_keys, l->keys, st, nl); s.up(l_mp, l->map_point, st, nl); s.up(l_outlier, l->outlier, st, nl); }
+    if (const int rc = s.check(c)) return rc;
     F.n = (int)nf;
-    UP(F.keys_un, f->keys_un, pslam_keypoint, nf); UP(F.u_right, f->u_right, float, nf); UP(F.desc, f->desc, uint8_t, nf * 32);
+    F.keys_un = s[f_keys]; F.u_right = s[f_ur]; F.desc = s[f_desc];
     std::memcpy(F.Tcw, f->Tcw, sizeof F.Tcw); F.Tcw_dev = nullptr; F.n_dev = nullptr;
     F.fx = f->fx; F.fy = f->fy; F.cx = f->cx; F.cy = f->cy; F.bf = f->bf; F.min_x = f->min_x; F.max_x = f->max_x; F.min_y = f->min_y; F.max_y = f->max_y;
     F.n_levels = f->n_levels; F.log_scale_factor = f->log_scale_factor;
     for (int i = 0; i < f->n_levels && i < PSLAM_MAX_LEVELS; ++i) F.scale[i] = f->scale_factors[i];
     F.inv_w = (float)SG_COLS / (f->max_x - f->min_x); F.inv_h = (float)SG_ROWS / (f->max_y - f->min_y);
     M.n = (int)nm;
-    UP(M.pos, m->pos, float, nm * 3); UP(M.normal, m->normal, float, nm * 3); UP(M.max_distance, m->max_distance, float, nm);
-    UP(M.min_distance, m->min_distance, float, nm); UP(M.desc, m->desc, uint8_t, nm * 32); UP(M.skip, m->skip, uint8_t, nm); UP(M.has_obs, m->has_obs, uint8_t, nm);
+    M.pos = s[m_pos]; M.normal = s[m_normal]; M.max_distance = s[m_maxd]; M.min_distance = s[m_mind]; M.desc = s[m_desc]; M.skip = s[m_skip]; M.has_obs = s[m_has_obs];
     if (l) {
         Ld.n = (int)nl;
-        UP(Ld.keys, l->keys, pslam_keypoint, nl); UP(Ld.map_point, l->map_point, int32_t, nl); UP(Ld.outlier, l->outlier, uint8_t, nl);
+        Ld.keys = s[l_keys]; Ld.map_point = s[l_mp]; Ld.outlier = s[l_outlier];
         std::memcpy(Ld.Tcw, l->Tcw, sizeof Ld.Tcw); Ld.Tcw_dev = nullptr; Ld.n_dev = nullptr;
     }
-#undef UP
     return PSLAM_OK;
 }
 
@@ -137,10 +129,6 @@ int pslam_search_by_projection_last(pslam_ctx* c, const pslam_frame_view* cur, c
 
 namespace pslam {
 void search_free(pslam_ctx* c) {
-    if (!c->search) return;
-    SearchBuffers& B = *c->search;
-    cudaFree(B.blob); cudaFree(B.d_cand); cudaFree(B.d_cand_n); cudaFree(B.d_cell_start); cudaFree(B.d_items); cudaFree(B.d_matches);
-    cudaFree(B.d_scalar); cudaFree(B.d_hist_idx); cudaFree(B.d_hist_bin); cudaFree(B.d_in_view);
     delete c->search;
     c->search = nullptr;
 }

@@ -50,25 +50,19 @@ int pslam_compute_stereo_from_rgbd_batch(pslam_ctx* c, const pslam_keypoint* key
     cudaStream_t st = c->stream;
     const size_t nf = (size_t)nframes, npx = (size_t)c->cfg.width * c->cfg.height;
     const bool same = keys_un == keys;
-    const size_t sz[] = {nf * cap * sizeof(pslam_keypoint), same ? 0 : nf * cap * sizeof(pslam_keypoint), nf * 4, nf * npx * 2, nf * cap * 4, nf * cap * 4};
-    const void* src[] = {keys, keys_un, n, depth};
-    size_t off[7]; off[0] = 0;
-    for (int i = 0; i < 6; ++i) off[i + 1] = (off[i] + sz[i] + 255) & ~(size_t)255;
-    uint8_t* d = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&d, off[6]));
-    cudaError_t e = cudaSuccess;
-    for (int i = 0; i < 4 && e == cudaSuccess; ++i) if (sz[i]) e = cudaMemcpyAsync(d + off[i], src[i], sz[i], cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) { cudaFree(d); return check_cuda(c, e, "stereo upload"); }
-    const int rc = pslam_compute_stereo_from_rgbd_batch_dev(c, (const pslam_keypoint*)(d + off[0]), (const pslam_keypoint*)(d + (same ? off[0] : off[1])),
-                                                            (const int32_t*)(d + off[2]), cap, (const uint16_t*)(d + off[3]), nframes, depth_factor, bf,
-                                                            (float*)(d + off[4]), (float*)(d + off[5]));
-    if (rc != PSLAM_OK) { cudaFree(d); return rc; }
-    e = cudaMemcpyAsync(u_right, d + off[4], sz[4], cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(depth_out, d + off[5], sz[5], cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    if (e != cudaSuccess) return check_cuda(c, e, "stereo");
-    return PSLAM_OK;
+    Slab s;
+    const auto d_keys = s.add<pslam_keypoint>(nf * cap), d_keys_un = s.add<pslam_keypoint>(same ? 0 : nf * cap);
+    const auto d_n = s.add<int32_t>(nf);
+    const auto d_depth = s.add<uint16_t>(nf * npx);
+    const auto d_ur = s.add<float>(nf * cap), d_dz = s.add<float>(nf * cap);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    s.up(d_keys, keys, st); s.up(d_keys_un, keys_un, st); s.up(d_n, n, st); s.up(d_depth, depth, st);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    rc = pslam_compute_stereo_from_rgbd_batch_dev(c, s[d_keys], s[same ? d_keys : d_keys_un], s[d_n], cap, s[d_depth], nframes, depth_factor, bf, s[d_ur], s[d_dz]);
+    if (rc != PSLAM_OK) return rc;
+    s.down(u_right, d_ur, st); s.down(depth_out, d_dz, st);
+    return s.sync(c, st);
 }
 
 }

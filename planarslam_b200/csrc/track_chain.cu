@@ -27,21 +27,21 @@ int orb_run_dev(pslam_ctx* c, const uint8_t* d_gray, int nframes, pslam_keypoint
 
 struct TrackBuffers {
     // map snapshot
-    void* map_blob = nullptr; size_t map_cap = 0; SearchMapDev M{}; uint8_t* d_skip = nullptr; uint8_t* d_skip0 = nullptr; int n_map = 0;
+    DevArray<uint8_t> map_blob; SearchMapDev M{}; DevArray<uint8_t> d_skip, d_skip0; int n_map = 0;
     // sequence products (stage A)
-    pslam_keypoint* d_kps = nullptr; uint8_t* d_desc = nullptr; int32_t* d_n = nullptr; float *d_ur = nullptr, *d_dz = nullptr; int cap_frames = 0, cap = 0;
+    DevArray<pslam_keypoint> d_kps; DevArray<uint8_t> d_desc; DevArray<int32_t> d_n; DevArray<float> d_ur, d_dz; int cap = 0;
     // chain state
-    float* d_T = nullptr;              // [3][16]: current pose, last pose, velocity
-    int32_t* d_matches = nullptr;      // [2][cap]: current / last frame's map point per key point
-    uint8_t* d_zero = nullptr;         // [cap] zeros (mvbOutlier of the last frame after the sweep)
+    DevArray<float> d_T;                 // [3][16]: current pose, last pose, velocity
+    DevArray<int32_t> d_matches;         // [2][cap]: current / last frame's map point per key point
+    DevArray<uint8_t> d_zero;            // [cap] zeros (mvbOutlier of the last frame after the sweep)
     // search scratch
-    int32_t *d_cell_start = nullptr, *d_items = nullptr, *d_cand_n = nullptr, *d_scalar = nullptr, *d_hist_idx = nullptr; uint32_t* d_cand = nullptr;
-    int8_t* d_hist_bin = nullptr; uint8_t* d_in_view = nullptr; size_t cap_pts = 0;
+    DevArray<int32_t> d_cell_start, d_items, d_cand_n, d_scalar, d_hist_idx; DevArray<uint32_t> d_cand;
+    DevArray<int8_t> d_hist_bin; DevArray<uint8_t> d_in_view;
     // pose problem
-    PoseHeaderDev* d_hdr = nullptr; float4* d_pa = nullptr; float4* d_pb = nullptr; uint8_t* d_level = nullptr; uint8_t* d_flags = nullptr;
-    PoseOutDev* d_out = nullptr; int32_t* d_kp_of_edge = nullptr; float* d_inv_sigma2 = nullptr;
+    DevArray<PoseHeaderDev> d_hdr; DevArray<float4> d_pa, d_pb; DevArray<uint8_t> d_level, d_flags;
+    DevArray<PoseOutDev> d_out; DevArray<int32_t> d_kp_of_edge; DevArray<float> d_inv_sigma2;
     // per-frame outputs
-    float* d_T_all = nullptr; int32_t* d_stats = nullptr;      // [n][16], [n][4] = matches / inliers after the motion-model stage and after the local-map stage
+    DevArray<float> d_T_all; DevArray<int32_t> d_stats;      // [n][16], [n][4] = matches / inliers after the motion-model stage and after the local-map stage
 };
 
 struct TrackCam { float fx, fy, cx, cy, bf; };
@@ -146,17 +146,7 @@ __global__ void __launch_bounds__(256) k_track_sweep(const PoseHeaderDev* __rest
     }
 }
 
-static void track_free_buffers(TrackBuffers& B) {
-    for (void* p : {B.map_blob, (void*)B.d_skip, (void*)B.d_skip0, (void*)B.d_kps, (void*)B.d_desc, (void*)B.d_n, (void*)B.d_ur, (void*)B.d_dz, (void*)B.d_T, (void*)B.d_matches,
-                    (void*)B.d_zero, (void*)B.d_cell_start, (void*)B.d_items, (void*)B.d_cand_n, (void*)B.d_scalar, (void*)B.d_hist_idx, (void*)B.d_cand, (void*)B.d_hist_bin,
-                    (void*)B.d_in_view, (void*)B.d_hdr, (void*)B.d_pa, (void*)B.d_pb, (void*)B.d_level, (void*)B.d_flags, (void*)B.d_out, (void*)B.d_kp_of_edge,
-                    (void*)B.d_inv_sigma2, (void*)B.d_T_all, (void*)B.d_stats})
-        if (p) cudaFree(p);
-}
-
 void track_free(pslam_ctx* c) {
-    if (!c->track) return;
-    track_free_buffers(*c->track);
     delete c->track;
     c->track = nullptr;
 }
@@ -175,30 +165,20 @@ int pslam_track_set_map(pslam_ctx* c, const pslam_map_points* m) {
     if (!c->track) c->track = new TrackBuffers();
     TrackBuffers& B = *c->track;
     const size_t nm = (size_t)m->n;
-    const size_t need = nm * (12 + 12 + 4 + 4 + 32 + 1 + 1) + 8 * 256;
-    if (need > B.map_cap) {
-        cudaFree(B.map_blob); cudaFree(B.d_skip); cudaFree(B.d_skip0);
-        B.map_blob = nullptr; B.d_skip = nullptr; B.d_skip0 = nullptr; B.map_cap = 0;
-        PSLAM_CUDA(c, cudaMalloc(&B.map_blob, need));
-        PSLAM_CUDA(c, cudaMalloc((void**)&B.d_skip, nm)); PSLAM_CUDA(c, cudaMalloc((void**)&B.d_skip0, nm));
-        B.map_cap = need;
-    }
-    uint8_t* p = (uint8_t*)B.map_blob;
+    Slab s;
+    const auto pos = s.add<float>(nm * 3), normal = s.add<float>(nm * 3), max_d = s.add<float>(nm), min_d = s.add<float>(nm);
+    const auto desc = s.add<uint8_t>(nm * 32), has_obs = s.add<uint8_t>(nm);
+    int rc;
+    B.n_map = 0;                // no snapshot until this one is uploaded
+    if ((rc = s.alloc(c, B.map_blob)) || (rc = B.d_skip.reserve(c, nm)) || (rc = B.d_skip0.reserve(c, nm))) return rc;
     cudaStream_t st = c->stream;
-    auto up = [&](const void* src, size_t bytes) -> void* {
-        void* d = p;
-        p += (bytes + 255) / 256 * 256;
-        cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, st);
-        return d;
-    };
-    B.M.n = m->n; B.n_map = m->n;
-    B.M.pos = (const float*)up(m->pos, nm * 12); B.M.normal = (const float*)up(m->normal, nm * 12);
-    B.M.max_distance = (const float*)up(m->max_distance, nm * 4); B.M.min_distance = (const float*)up(m->min_distance, nm * 4);
-    B.M.desc = (const uint8_t*)up(m->desc, nm * 32); B.M.has_obs = (const uint8_t*)up(m->has_obs, nm);
+    s.up(pos, m->pos, st); s.up(normal, m->normal, st); s.up(max_d, m->max_distance, st); s.up(min_d, m->min_distance, st);
+    s.up(desc, m->desc, st); s.up(has_obs, m->has_obs, st);
     PSLAM_CUDA(c, cudaMemcpyAsync(B.d_skip0, m->skip, nm, cudaMemcpyHostToDevice, st));
+    B.M.n = m->n; B.n_map = m->n;
+    B.M.pos = s[pos]; B.M.normal = s[normal]; B.M.max_distance = s[max_d]; B.M.min_distance = s[min_d]; B.M.desc = s[desc]; B.M.has_obs = s[has_obs];
     B.M.skip = B.d_skip;
-    PSLAM_CUDA(c, cudaStreamSynchronize(st));       // the caller's arrays may be pageable
-    return PSLAM_OK;
+    return s.sync(c, st);       // the caller's arrays may be pageable
 }
 
 int pslam_track_sequence_dev(pslam_ctx* c, const uint8_t* d_gray, const uint16_t* d_depth, int nframes, const pslam_track_params* prm, const float* Tcw0,
@@ -211,29 +191,27 @@ int pslam_track_sequence_dev(pslam_ctx* c, const uint8_t* d_gray, const uint16_t
     const OrbGeom& g = c->geom;
     const int cap = std::min(pslam_orb_max_keypoints(c), SEARCH_MAX_KP);
     cudaStream_t st = c->stream;
-#define TA(ptr, bytes) do { if (ptr) cudaFree(ptr); ptr = nullptr; PSLAM_CUDA(c, cudaMalloc((void**)&(ptr), (bytes))); } while (0)
-    if (nframes > B.cap_frames || cap != B.cap) {
-        TA(B.d_kps, (size_t)nframes * cap * sizeof(pslam_keypoint)); TA(B.d_desc, (size_t)nframes * cap * 32); TA(B.d_n, (size_t)nframes * 4);
-        TA(B.d_ur, (size_t)nframes * cap * 4); TA(B.d_dz, (size_t)nframes * cap * 4); TA(B.d_T_all, (size_t)nframes * 64); TA(B.d_stats, (size_t)nframes * 16);
-        B.cap_frames = nframes;
-    }
+    const size_t nf = (size_t)nframes;
+    int rc;
+    if ((rc = B.d_kps.reserve(c, nf * cap)) || (rc = B.d_desc.reserve(c, nf * cap * 32)) || (rc = B.d_n.reserve(c, nf)) || (rc = B.d_ur.reserve(c, nf * cap)) ||
+        (rc = B.d_dz.reserve(c, nf * cap)) || (rc = B.d_T_all.reserve(c, nf * 16)) || (rc = B.d_stats.reserve(c, nf * 4)))
+        return rc;
     if (cap != B.cap) {
-        TA(B.d_T, 3 * 64); TA(B.d_matches, (size_t)2 * cap * 4); TA(B.d_zero, cap); TA(B.d_cell_start, (SG_CELLS + 1) * 4); TA(B.d_items, SEARCH_MAX_KP * 4);
-        TA(B.d_scalar, 16); TA(B.d_hdr, sizeof(PoseHeaderDev)); TA(B.d_pa, (size_t)cap * sizeof(float4)); TA(B.d_pb, (size_t)cap * sizeof(float4)); TA(B.d_level, cap);
-        TA(B.d_flags, cap); TA(B.d_out, sizeof(PoseOutDev)); TA(B.d_kp_of_edge, (size_t)cap * 4); TA(B.d_inv_sigma2, PSLAM_MAX_LEVELS * 4);
+        if ((rc = B.d_T.reserve(c, 3 * 16)) || (rc = B.d_matches.reserve(c, (size_t)2 * cap)) || (rc = B.d_zero.reserve(c, cap)) ||
+            (rc = B.d_cell_start.reserve(c, SG_CELLS + 1)) || (rc = B.d_items.reserve(c, SEARCH_MAX_KP)) || (rc = B.d_scalar.reserve(c, 4)) ||
+            (rc = B.d_hdr.reserve(c, 1)) || (rc = B.d_pa.reserve(c, cap)) || (rc = B.d_pb.reserve(c, cap)) || (rc = B.d_level.reserve(c, cap)) ||
+            (rc = B.d_flags.reserve(c, cap)) || (rc = B.d_out.reserve(c, 1)) || (rc = B.d_kp_of_edge.reserve(c, cap)) || (rc = B.d_inv_sigma2.reserve(c, PSLAM_MAX_LEVELS)))
+            return rc;
         PSLAM_CUDA(c, cudaMemsetAsync(B.d_zero, 0, cap, st));
         PSLAM_CUDA(c, cudaMemcpyAsync(B.d_inv_sigma2, c->inv_sigma2.data(), g.nlevels * 4, cudaMemcpyHostToDevice, st));
         B.cap = cap;
     }
     const size_t npts = (size_t)std::max(B.n_map, cap);
-    if (npts > B.cap_pts) {
-        TA(B.d_cand, npts * SEARCH_CAND_CAP * 4); TA(B.d_cand_n, npts * 4); TA(B.d_hist_idx, npts * 4); TA(B.d_hist_bin, npts); TA(B.d_in_view, npts);
-        B.cap_pts = npts;
-    }
-#undef TA
+    if ((rc = B.d_cand.reserve(c, npts * SEARCH_CAND_CAP)) || (rc = B.d_cand_n.reserve(c, npts)) || (rc = B.d_hist_idx.reserve(c, npts)) ||
+        (rc = B.d_hist_bin.reserve(c, npts)) || (rc = B.d_in_view.reserve(c, npts)))
+        return rc;
     // ---- stage A: ORB + stereo association for every frame of the sequence ----
-    int rc = orb_run_dev(c, d_gray, nframes, B.d_kps, B.d_desc, cap, B.d_n);
-    if (rc != PSLAM_OK) return rc;
+    if ((rc = orb_run_dev(c, d_gray, nframes, B.d_kps, B.d_desc, cap, B.d_n)) != PSLAM_OK) return rc;
     if ((rc = pslam_compute_stereo_from_rgbd_batch_dev(c, B.d_kps, B.d_kps, B.d_n, cap, d_depth, nframes, prm->depth_factor, prm->bf, B.d_ur, B.d_dz)) != PSLAM_OK) return rc;
     // ---- stage B ----
     PSLAM_CUDA(c, cudaMemcpyAsync(B.d_T, Tcw0, 64, cudaMemcpyHostToDevice, st));
@@ -300,16 +278,16 @@ int pslam_track_sequence(pslam_ctx* c, const uint8_t* gray, const uint16_t* dept
     if (!gray || !depth || nframes < 1) return set_error(c, PSLAM_E_INVALID, "bad tracking arguments");
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     const size_t npx = (size_t)c->cfg.width * c->cfg.height;
-    uint8_t* dg = nullptr; uint16_t* dd = nullptr;
-    PSLAM_CUDA(c, cudaMalloc((void**)&dg, (size_t)nframes * npx));
-    cudaError_t e = cudaMalloc((void**)&dd, (size_t)nframes * npx * 2);
-    if (e != cudaSuccess) { cudaFree(dg); return check_cuda(c, e, "cudaMalloc(track)"); }
-    cudaMemcpyAsync(dg, gray, (size_t)nframes * npx, cudaMemcpyHostToDevice, c->stream);
-    cudaMemcpyAsync(dd, depth, (size_t)nframes * npx * 2, cudaMemcpyHostToDevice, c->stream);
-    const int rc = pslam_track_sequence_dev(c, dg, dd, nframes, prm, Tcw0, Tcw_out, stats_out);
-    cudaStreamSynchronize(c->stream);
-    cudaFree(dg); cudaFree(dd);
-    return rc;
+    Slab s;
+    const auto dg = s.add<uint8_t>((size_t)nframes * npx);
+    const auto dd = s.add<uint16_t>((size_t)nframes * npx);
+    int rc = s.alloc(c);
+    if (rc != PSLAM_OK) return rc;
+    s.up(dg, gray, c->stream); s.up(dd, depth, c->stream);
+    if ((rc = s.check(c)) != PSLAM_OK) return rc;
+    rc = pslam_track_sequence_dev(c, s[dg], s[dd], nframes, prm, Tcw0, Tcw_out, stats_out);
+    const int src = s.sync(c, c->stream);
+    return rc != PSLAM_OK ? rc : src;
 }
 
 }  // extern "C"
