@@ -260,6 +260,69 @@ int pslam_track_sequence_dev(pslam_ctx* ctx, const uint8_t* d_gray, const uint16
 int pslam_track_sequence(pslam_ctx* ctx, const uint8_t* gray, const uint16_t* depth, int nframes, const pslam_track_params* params, const float* Tcw0,
                          float* Tcw_out, int32_t* stats /* may be NULL */);
 
+/* ---- Device-resident PLANAR tracking chain: what PlanarSLAM's Tracking::Track() does per frame (src/Tracking.cc:239-318) -------------------------
+ *   frame products (batched over the sequence): ORB + ComputeStereoFromRGBD; ExtractLineSegment + LBD + isLineGood; ComputePlanes + surface normals
+ *   TrackManhattanFrame(mLastRcm, vSurfaceNormal, mVF3DLines)    :247-254      R_cw = (Rotation_cm * MF_can^T)^T, mLastRcm = MF_can
+ *   TranslationWithMotionModel()                                 :1739-1859    SetPose(mVelocity * mLastFrame.mTcw); SearchByProjection(cur, last, 15) and, below
+ *                                                                              50 matches, MatchORBPoints; LSDmatcher::SearchByDescriptor(mpReferenceKF, cur);
+ *                                                                              SearchMapByCoefficients; fail below 10 matches; R_cw into mTcw;
+ *                                                                              TranslationOptimization (point, line, plane edges); outliers dropped; fail when
+ *                                                                              nmatchesMap < 3 or all inliers < 3 (pose back to mVelocity * mLastFrame.mTcw)
+ *   TrackLocalMap()                                              :1954-2046    SearchLocalPoints, SearchLocalLines (isInFrustum(MapLine*, 0.6) + LSDmatcher::
+ *                                                                              SearchByProjection), SearchMapByCoefficients, PoseOptimization (point, line,
+ *                                                                              plane, parallel, vertical edges); fail below 7 inliers (mnMatchesInliers)
+ *   mLastRcm from the final pose (:281-284); mVelocity when the frame tracked (:310-318); "Clean VO matches" (points without observations dropped).
+ * Conventions:
+ *   - frame 0 runs TrackManhattanFrame(Rcm0) (its result becomes mLastRcm, as in StereoInitialization, :224-230) and TrackLocalMap from Tcw0;
+ *     frames t >= 1 run the body of Track() above.  Frame 1 predicts with vel0 (NULL: identity).
+ *   - a frame whose motion-model stage fails is flagged, keeps the pose mVelocity * mLastFrame.mTcw, skips TrackLocalMap and leaves mVelocity alone;
+ *     the reference's TranslationEstimation / Relocalization after such a failure are not modelled.  A frame whose local-map stage fails is flagged and
+ *     leaves mVelocity alone.
+ *   - SearchMapByCoefficients only writes the associations it finds: the local-map call keeps the motion-model stage's plane / parallel / vertical
+ *     associations it does not replace (src/PlaneMatcher.cpp:36-58).
+ *   - the chain does not stop at a failed frame: the following frames are tracked from the kept pose.
+ *   - the last frame's map points for SearchByProjection(cur, last) / MatchORBPoints are the frame's matches at the end of the frame with the
+ *     local-map outliers flagged (mvbOutlier), as the reference's mLastFrame holds them.
+ *   - not modelled: key-frame insertion, MapPlane::UpdateCoefficientsAndPoints / FlagMatchedPlanePoints between frames (:294-303), UpdateLastFrame's
+ *     reference-key-frame pose, the mnLastRelocFrameId + 2 window sizes; the snapshot (map, reference key frame, Rotation_cm) is fixed for the sequence.
+ * The snapshot is uploaded once by pslam_track_set_planar_map into state of its own (what pslam_track_set_map uploaded is left alone).  Stage B runs
+ * frame after frame on the context's stream with no host synchronisation and no device-to-host copy between frames: every branch is taken on the device.
+ * Outputs: Tcw_out [nframes][16]; Rcm_out [nframes][9] = mLastRcm after each frame (may be NULL); stats [nframes][PSLAM_PLANAR_STATS] (may be NULL). */
+typedef struct pslam_map_lines {
+    int32_t n; const double* pos /* [n][6] GetWorldPos: start, end */; const double* normal /* [n][3] */;
+    const float *max_distance, *min_distance;      /* raw mfMaxDistance / mfMinDistance (the 1.2 / 0.8 factors are applied by the frustum test) */
+    const uint8_t* desc /* [n][32] GetDescriptor */; const uint8_t* skip /* isBad */; const uint8_t* has_obs /* Observations() > 0 */;
+} pslam_map_lines;
+typedef struct pslam_map_planes {
+    int32_t n; const float* coef /* [n][4] GetWorldPos */; const uint8_t* bad /* [n] isBad */;
+    const int32_t* pts_off /* [n + 1] */; const float* pts /* [pts_off[n]][3] mvPlanePoints */;
+} pslam_map_planes;
+typedef struct pslam_planar_map {
+    pslam_map_points points; pslam_map_lines lines; pslam_map_planes planes;
+    int32_t n_ref_lines;                           /* mpReferenceKF's key lines (SearchByDescriptor): */
+    const uint8_t* ref_line_desc;                  /*   [n_ref_lines][32] mLineDescriptors */
+    const int32_t* ref_line_map;                   /*   [n_ref_lines] index into lines of GetMapLineMatches()[i], -1 for NULL */
+    float R_cm[9];                                 /* Rotation_cm, the map's Manhattan frame (row-major) */
+} pslam_planar_map;
+typedef struct pslam_planar_track_params {
+    pslam_track_params base;                       /* camera, windows of the point searches, use_motion_model is ignored (always the motion model) */
+    float line_th;                                 /* th of SearchLocalLines' LSDmatcher::SearchByProjection: 1 (:2368-2375) */
+    float line_nnratio;                            /* LSDmatcher's mfNNratio (0.6) */
+    float plane_dist_ref, plane_ang_ref, plane_ver_th, plane_par_th;   /* Plane.AssociationDisRef, AssociationAngRef, VerticalThreshold, ParallelThreshold */
+    double angle_info, dist_info, par_info, ver_info, plane_chi, vp_chi; /* Plane.AngleInfo, DistanceInfo, ParallelInfo, VerticalInfo, Chi, VPChi */
+    float plane_dist_th;                           /* Plane.DistanceThreshold (ComputePlanes) */
+    int32_t max_lines;                             /* key lines kept per frame (40), <= 64 */
+    uint32_t line_seed;                            /* srand seed of isLineGood's RANSAC, every frame */
+} pslam_planar_track_params;
+/* stats row: motion-model stage {point matches (SearchByProjection or MatchORBPoints), line matches, plane matches, MatchORBPoints ran, nmatchesMap, ok},
+ * local-map stage {point, line, plane, parallel, vertical edges of PoseOptimization, mnMatchesInliers, ok}.  Frame 0's motion-model entries are 0. */
+#define PSLAM_PLANAR_STATS 13
+int pslam_track_set_planar_map(pslam_ctx* ctx, const pslam_planar_map* map);
+int pslam_track_planar_sequence_dev(pslam_ctx* ctx, const uint8_t* d_gray, const uint16_t* d_depth, int nframes, const pslam_planar_track_params* params,
+                                    const float* Tcw0, const float* vel0 /* may be NULL */, const float* Rcm0, float* Tcw_out, float* Rcm_out, int32_t* stats);
+int pslam_track_planar_sequence(pslam_ctx* ctx, const uint8_t* gray, const uint16_t* depth, int nframes, const pslam_planar_track_params* params,
+                                const float* Tcw0, const float* vel0, const float* Rcm0, float* Tcw_out, float* Rcm_out, int32_t* stats);
+
 /* ---- Key-frame descriptor exchange over NVLink peer memory, fused with the Hamming matcher (SURVEY.md section 8e) -------------------
  * The one exchange step of the multi-GPU layout: every rank (one process per GPU) publishes the ORB block of a key frame - descriptors [n][32], key points
  * [n] (28 B), count - into a record in ITS OWN HBM; peers map the records through CUDA IPC (NVLink / NVSwitch P2P) and pslam_exchange_match_dev finds, for

@@ -79,6 +79,14 @@ __global__ void __launch_bounds__(32) k_line_search(int nf, const float* __restr
     if (lane == 0) *nmatches = count;
 }
 
+int line_search_run_dev(pslam_ctx* c, int nf, const float* pt, const float* angle, const int32_t* octave, const uint8_t* desc, const uint8_t* has_obs, const float* scale,
+                        int n_levels, int nm, const uint8_t* skip, const int32_t* level, const float* view_cos, const float* proj, const uint8_t* mdesc,
+                        const uint8_t* m_has_obs, float th, float nnratio, int32_t* assigned, int32_t* nmatches) {
+    PSLAM_LAUNCH(c, "line_search", k_line_search<<<1, 32, 0, c->stream>>>(nf, pt, angle, octave, desc, has_obs, scale, n_levels, nm, skip, level, view_cos, proj, mdesc,
+                 m_has_obs, th, nnratio, assigned, nmatches));
+    return PSLAM_OK;
+}
+
 }  // namespace pslam
 
 using namespace pslam;
@@ -111,8 +119,8 @@ extern "C" int pslam_line_search_by_projection(pslam_ctx* c, int nf, const float
     s.up(d_pt, pt, st); s.up(d_angle, angle, st); s.up(d_octave, octave, st); s.up(d_desc, desc, st); s.up(d_has_obs, has_obs, st); s.up(d_scale, scale_factors, st);
     s.up(d_skip, skip, st); s.up(d_level, level, st); s.up(d_view_cos, view_cos, st); s.up(d_proj, proj, st); s.up(d_mdesc, mdesc, st); s.up(d_m_has_obs, m_has_obs, st);
     if ((rc = s.check(c)) != PSLAM_OK) return rc;
-    PSLAM_LAUNCH(c, "line_search", k_line_search<<<1, 32, 0, st>>>(nf, s[d_pt], s[d_angle], s[d_octave], s[d_desc], s[d_has_obs], s[d_scale], n_levels, nm, s[d_skip],
-                 s[d_level], s[d_view_cos], s[d_proj], s[d_mdesc], s[d_m_has_obs], th, nnratio, s[d_assigned], s[d_n]));
+    line_search_run_dev(c, nf, s[d_pt], s[d_angle], s[d_octave], s[d_desc], s[d_has_obs], s[d_scale], n_levels, nm, s[d_skip], s[d_level], s[d_view_cos], s[d_proj],
+                        s[d_mdesc], s[d_m_has_obs], th, nnratio, s[d_assigned], s[d_n]);
     int32_t n = 0;
     s.down(assigned, d_assigned, st); s.down(&n, d_n, st);
     if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;

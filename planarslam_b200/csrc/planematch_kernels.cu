@@ -46,6 +46,15 @@ __global__ void k_plane_assign(int n_frame, int n_map, const uint8_t* __restrict
     if (m >= 0) atomicAdd(nmatches, 1);
 }
 
+// pM: the frame planes in world coordinates ([n_frame][4]); ang / mind: [n_frame][n_map] scratch; *nmatches is incremented per matched frame plane
+int plane_match_run_dev(pslam_ctx* c, int n_frame, int n_map, const float* pM, const float* map_coef, const uint8_t* map_bad, const int32_t* pts_off, const float* pts,
+                        float* ang, float* mind, float dTh, float aTh, float verTh, float parTh, int32_t* match, int32_t* ver, int32_t* par, int32_t* nmatches) {
+    PSLAM_LAUNCH(c, "plane_pairs", k_plane_pairs<<<(n_frame * n_map + 7) / 8, 256, 0, c->stream>>>(n_frame, n_map, pM, map_coef, pts_off, pts, ang, mind));
+    PSLAM_LAUNCH(c, "plane_assign", k_plane_assign<<<(n_frame + 63) / 64, 64, 0, c->stream>>>(n_frame, n_map, map_bad, ang, mind, dTh, aTh, verTh, parTh, match, ver, par,
+                 nmatches));
+    return PSLAM_OK;
+}
+
 }  // namespace pslam
 
 using namespace pslam;
@@ -81,9 +90,8 @@ extern "C" int pslam_plane_match(pslam_ctx* c, const float* Tcw, int n_frame, co
     s.zero(d_cnt, st);
     if ((rc = s.check(c)) != PSLAM_OK) return rc;
     int32_t* out_d = s[d_out];
-    PSLAM_LAUNCH(c, "plane_pairs", k_plane_pairs<<<(n_frame * n_map + 7) / 8, 256, 0, st>>>(n_frame, n_map, s[d_pM], s[d_mc], s[d_off], s[d_pts], s[d_ang], s[d_min]));
-    PSLAM_LAUNCH(c, "plane_assign", k_plane_assign<<<(n_frame + 63) / 64, 64, 0, st>>>(n_frame, n_map, s[d_bad], s[d_ang], s[d_min], dTh, aTh, verTh, parTh, out_d,
-                 out_d + n_frame, out_d + 2 * n_frame, s[d_cnt]));
+    plane_match_run_dev(c, n_frame, n_map, s[d_pM], s[d_mc], s[d_bad], s[d_off], s[d_pts], s[d_ang], s[d_min], dTh, aTh, verTh, parTh, out_d, out_d + n_frame,
+                        out_d + 2 * n_frame, s[d_cnt]);
     std::vector<int32_t> out((size_t)3 * n_frame + 1);
     s.down(out.data(), d_out, st); s.down(out.data() + 3 * n_frame, d_cnt, st);
     if ((rc = s.sync(c, st)) != PSLAM_OK) return rc;

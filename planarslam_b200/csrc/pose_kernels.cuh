@@ -20,22 +20,9 @@
 
 #include "pslam_internal.h"
 #include "geom_device.cuh"
+#include "pose_records.h"
 
 namespace pslam {
-
-enum { PK_MONO = 0, PK_STEREO = 1, PK_LINE = 2, PK_PLANE = 3, PK_PAR = 4, PK_VER = 5,
-       PK_MONO_T = 6, PK_STEREO_T = 7, PK_LINE_T = 8, PK_PLANE_T = 9 };   // translation-only variants (TranslationOptimization)
-
-// A problem's edges are numbered points first, then the start / end edge of every line, then the plane, parallel-plane
-// and vertical-plane edges.  Point edge i is two float4 records (every field is a float in the reference's Frame, so
-// widening on load gives the same doubles): pt_a[edge_off + i] = (Xw, u), pt_b[edge_off + i] = (v, uR, inv_sigma2, Huber
-// delta); uR < 0 makes it monocular.  Line and plane edges are PoseEdgeDev records, wide[wide_off + i - n_pt].
-struct PoseEdgeDev {            // 104 bytes
-    int32_t kind, idx;          // idx: index inside its family (line i / plane i)
-    double a[8];                // lines: Xw[3], obs[3]; planes: world plane[4], measured plane[4] (normalised)
-    double info[3];
-    double delta;               // Huber delta
-};
 
 struct PoseHeaderDev {
     int32_t edge_off, n_edges;  // first edge in the point records and the level bytes, edge count

@@ -24,16 +24,6 @@ struct PoseBuffers {
     std::vector<uint8_t> h_flags[5];
 };
 
-static void plane_from_float4(const float* v, double out[4]) {     // Converter::toPlane3D + Plane3D::normalize
-    double p[4] = {v[0], v[1], v[2], v[3]};
-    if (v[3] < 0.0f) for (int i = 0; i < 4; ++i) p[i] = -p[i];
-    const double n = std::sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]);
-    const double s = 1. / n;
-    for (int i = 0; i < 4; ++i) p[i] = p[i] * s;
-    if (p[3] < 0.0) for (int i = 0; i < 4; ++i) p[i] = -p[i];
-    for (int i = 0; i < 4; ++i) out[i] = p[i];
-}
-
 int pose_pack_upload(pslam_ctx* c, const pslam_pose_problem* probs, int n, const float* Tcw0, int mode) {
     if (!c->pose) c->pose = new PoseBuffers();
     PoseBuffers& B = *c->pose;
@@ -54,59 +44,30 @@ int pose_pack_upload(pslam_ctx* c, const pslam_pose_problem* probs, int n, const
         H.n_initial = mode == 0 ? P.n_points + P.n_lines + P.n_planes + P.n_par + P.n_ver : P.n_points;   // :3137-3139, :3245-3246
         H.mode = mode;
         const float* T0 = Tcw0 + 16 * p;
-        // R_cw * X as cv::Mat(CV_32F) products do it: double accumulation, float result (TranslationOptimization :3019,:3066,:3161)
-        auto rot_f = [&](double x, double y, double z, int row) -> double {
-            return (double)(float)((double)T0[row * 4 + 0] * (double)(float)x + (double)T0[row * 4 + 1] * (double)(float)y + (double)T0[row * 4 + 2] * (double)(float)z);
-        };
         H.fx = P.fx; H.fy = P.fy; H.cx = P.cx; H.cy = P.cy; H.bf = P.bf; H.plane_chi = P.plane_chi; H.vp_chi = P.vp_chi;
-        std::memcpy(H.Tcw0, Tcw0 + 16 * p, sizeof H.Tcw0);
-        const float deltaMono = std::sqrt(5.991), deltaStereo = std::sqrt(7.815);       // const float in the reference (:583-584)
-        const float deltaPlane = std::sqrt(P.plane_chi), deltaVP = std::sqrt(P.vp_chi);
-        const double angleInfo = 3282.8 / (P.angle_info * P.angle_info), disInfo = P.dist_info * P.dist_info;
-        const double parInfo = 3282.8 / (P.par_info * P.par_info), verInfo = 3282.8 / (P.ver_info * P.ver_info);
-        for (int i = 0; i < P.n_points; ++i) {     // monocular when uR < 0; every field is a float, so the float record loses nothing
-            const bool mono = P.obs[3 * i + 2] < 0;
-            float X[3];
-            for (int k = 0; k < 3; ++k) X[k] = mode == 0 ? P.Xw[3 * i + k] : (float)rot_f(P.Xw[3 * i], P.Xw[3 * i + 1], P.Xw[3 * i + 2], k);
-            B.h_pa.push_back(make_float4(X[0], X[1], X[2], P.obs[3 * i]));
-            B.h_pb.push_back(make_float4(P.obs[3 * i + 1], P.obs[3 * i + 2], P.inv_sigma2[i], mono ? deltaMono : deltaStereo));
+        std::memcpy(H.Tcw0, T0, sizeof H.Tcw0);
+        const PoseEdgeConsts K = pose_edge_consts(P.angle_info, P.dist_info, P.par_info, P.ver_info, P.plane_chi, P.vp_chi);
+        for (int i = 0; i < P.n_points; ++i) {
+            float4 a, b;
+            pose_point_record(P.Xw + 3 * i, P.obs[3 * i], P.obs[3 * i + 1], P.obs[3 * i + 2], P.inv_sigma2[i], mode, T0, a, b);
+            B.h_pa.push_back(a); B.h_pb.push_back(b);
         }
         auto add_wide = [&](const PoseEdgeDev& e) {
             B.h_wide.push_back(e);
             B.h_pa.push_back(make_float4(0, 0, 0, 0)); B.h_pb.push_back(make_float4(0, 0, 0, 0));
         };
+        PoseEdgeDev e;
         for (int i = 0; i < P.n_lines; ++i)
-            for (int s = 0; s < 2; ++s) {
-                PoseEdgeDev e;
-                std::memset(&e, 0, sizeof e);
-                e.kind = mode == 0 ? PK_LINE : PK_LINE_T; e.idx = i;
-                const double* X = P.line_Xw + 6 * i + 3 * s;
-                for (int k = 0; k < 3; ++k) { e.a[k] = mode == 0 ? X[k] : rot_f(X[0], X[1], X[2], k); e.a[3 + k] = P.line_obs[3 * i + k]; e.info[k] = 1.0; }
-                e.delta = deltaStereo;
-                add_wide(e);
-            }
-        auto add_planes = [&](int kind, int cnt, const float* meas, const float* map, double i0, double i1, double i2, double delta) {
-            for (int i = 0; i < cnt; ++i) {
-                PoseEdgeDev e;
-                std::memset(&e, 0, sizeof e);
-                e.kind = kind; e.idx = i;
-                plane_from_float4(map + 4 * i, e.a); plane_from_float4(meas + 4 * i, e.a + 4);
-                e.info[0] = i0; e.info[1] = i1; e.info[2] = i2; e.delta = delta;
-                add_wide(e);
-            }
+            for (int s = 0; s < 2; ++s) { pose_line_record(P.line_Xw + 6 * i, P.line_obs + 3 * i, i, s, mode, T0, e); add_wide(e); }
+        auto add_planes = [&](int kind, int cnt, const float* meas, const float* map) {
+            for (int i = 0; i < cnt; ++i) { pose_plane_record(kind, i, map + 4 * i, meas + 4 * i, T0, K, e); add_wide(e); }
         };
         if (mode == 0) {
-            add_planes(PK_PLANE, P.n_planes, P.plane_meas, P.plane_map, angleInfo, angleInfo, disInfo, deltaPlane);
-            add_planes(PK_PAR, P.n_par, P.par_meas, P.par_map, parInfo, parInfo, 0, deltaVP);
-            add_planes(PK_VER, P.n_ver, P.ver_meas, P.ver_map, verInfo, verInfo, 0, deltaVP);
+            add_planes(PK_PLANE, P.n_planes, P.plane_meas, P.plane_map);
+            add_planes(PK_PAR, P.n_par, P.par_meas, P.par_map);
+            add_planes(PK_VER, P.n_ver, P.ver_meas, P.ver_map);
         } else if (P.n_points >= 3) {          // the reference returns before adding planes when < 3 points are matched (:3198-3200)
-            const size_t first = B.h_wide.size();
-            add_planes(PK_PLANE_T, P.n_planes, P.plane_meas, P.plane_map, angleInfo, angleInfo, disInfo, deltaPlane);
-            for (size_t k = first; k < B.h_wide.size(); ++k) {     // Xw.rotateNormal(toMatrix3d(R_cw)): widened float rotation, not renormalised
-                double* a = B.h_wide[k].a;
-                const double nrm[3] = {a[0], a[1], a[2]};
-                for (int r = 0; r < 3; ++r) a[r] = (double)T0[r * 4 + 0] * nrm[0] + (double)T0[r * 4 + 1] * nrm[1] + (double)T0[r * 4 + 2] * nrm[2];
-            }
+            add_planes(PK_PLANE_T, P.n_planes, P.plane_meas, P.plane_map);
         }
         H.n_edges = (int)B.h_pa.size() - H.edge_off;
         n_plane_edges += H.n_edges - H.n_pt - 2 * H.n_line;

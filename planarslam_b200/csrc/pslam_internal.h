@@ -82,6 +82,7 @@ struct SearchBuffers;
 struct LbaBuffers;
 struct LsdBuffers;
 struct TrackBuffers;
+struct PlanarTrackBuffers;
 struct ExchangeBuffers;
 struct PlanePostBuffers;
 struct BowDbBuffers;
@@ -146,6 +147,7 @@ struct pslam_ctx {
     pslam::LbaBuffers* lba = nullptr;            // local bundle adjustment staging (lba_pipeline.cu)
     pslam::LsdBuffers* lsd = nullptr;            // line-segment detector buffers (lsd_pipeline.cu)
     pslam::TrackBuffers* track = nullptr;        // device-resident tracking chain (track_chain.cu)
+    pslam::PlanarTrackBuffers* ptrack = nullptr; // device-resident planar tracking chain (track_chain.cu)
     pslam::PlanePostBuffers* planepost = nullptr; // Frame::ComputePlanes post-processing + surface normals (planepost_kernels.cu)
     pslam::FrameBuffers* frame = nullptr;        // staging of pslam_frame_construct_batch (frame_pipeline.cu)
     pslam::BowDbBuffers* bowdb = nullptr;        // key-frame database BowVectors for loop / relocalisation candidates (bow_kernels.cu)
@@ -164,6 +166,13 @@ int orb_build_geometry(pslam_ctx* c);
 int orb_alloc(pslam_ctx* c);
 int orb_run_dev(pslam_ctx* c, const uint8_t* d_gray, int nframes, pslam_keypoint* d_kps, uint8_t* d_desc, int cap,
                 int32_t* d_n);
+// device-pointer launchers of the per-function kernels, for the tracking chains (track_chain.cu); enqueue on the context's stream
+int line_search_run_dev(pslam_ctx* c, int nf, const float* pt, const float* angle, const int32_t* octave, const uint8_t* desc, const uint8_t* has_obs, const float* scale,
+                        int n_levels, int nm, const uint8_t* skip, const int32_t* level, const float* view_cos, const float* proj, const uint8_t* mdesc,
+                        const uint8_t* m_has_obs, float th, float nnratio, int32_t* assigned, int32_t* nmatches);   // linesearch_kernels.cu
+int plane_match_run_dev(pslam_ctx* c, int n_frame, int n_map, const float* pM, const float* map_coef, const uint8_t* map_bad, const int32_t* pts_off, const float* pts,
+                        float* ang, float* mind, float dTh, float aTh, float verTh, float parTh, int32_t* match, int32_t* ver, int32_t* par,
+                        int32_t* nmatches);                                                                                   // planematch_kernels.cu
 // pose optimisation (pose_pipeline.cu)
 void pose_free(pslam_ctx* c);
 void search_free(pslam_ctx* c);

@@ -49,3 +49,87 @@ class Tracker:
         self.ctx.check(self.ctx.L.pslam_track_sequence(self.ctx.h, g.ctypes.data, d.ctypes.data, n, C.byref(self.params), T0.ctypes.data, poses.ctypes.data,
                                                        stats.ctypes.data))
         return poses, stats
+
+
+class MapLinesC(C.Structure):
+    _fields_ = [("n", C.c_int32), ("pos", C.c_void_p), ("normal", C.c_void_p), ("max_distance", C.c_void_p), ("min_distance", C.c_void_p),
+                ("desc", C.c_void_p), ("skip", C.c_void_p), ("has_obs", C.c_void_p)]
+
+
+class MapPlanesC(C.Structure):
+    _fields_ = [("n", C.c_int32), ("coef", C.c_void_p), ("bad", C.c_void_p), ("pts_off", C.c_void_p), ("pts", C.c_void_p)]
+
+
+class PlanarMapC(C.Structure):
+    _fields_ = [("points", MapPointsC), ("lines", MapLinesC), ("planes", MapPlanesC), ("n_ref_lines", C.c_int32), ("ref_line_desc", C.c_void_p),
+                ("ref_line_map", C.c_void_p), ("R_cm", C.c_float * 9)]
+
+
+class PlanarTrackParams(C.Structure):
+    _fields_ = [("base", TrackParams), ("line_th", C.c_float), ("line_nnratio", C.c_float), ("plane_dist_ref", C.c_float), ("plane_ang_ref", C.c_float),
+                ("plane_ver_th", C.c_float), ("plane_par_th", C.c_float), ("angle_info", C.c_double), ("dist_info", C.c_double), ("par_info", C.c_double),
+                ("ver_info", C.c_double), ("plane_chi", C.c_double), ("vp_chi", C.c_double), ("plane_dist_th", C.c_float), ("max_lines", C.c_int32),
+                ("line_seed", C.c_uint32)]
+
+
+PLANAR_STATS = 13      # PSLAM_PLANAR_STATS
+PLANAR_STATS_FIELDS = ("mm_points", "mm_lines", "mm_planes", "mm_fallback", "mm_map_inliers", "mm_ok",
+                       "lm_points", "lm_lines", "lm_planes", "lm_parallel", "lm_vertical", "lm_inliers", "lm_ok")
+
+
+def default_planar_params(width=640, height=480, **kw) -> PlanarTrackParams:
+    """TUM3.yaml: Plane.AssociationDisRef 0.05, AssociationAngRef 0.985, VerticalThreshold 0.08716, ParallelThreshold 0.98481, DistanceThreshold 0.05;
+    the pose-optimisation plane settings of synth_pose.PLANE_SETTINGS; 40 key lines, srand seed 1."""
+    from .synth_pose import PLANE_SETTINGS
+    p = PlanarTrackParams(default_params(width=width, height=height), 1.0, 0.6, 0.05, 0.985, 0.08716, 0.98481, PLANE_SETTINGS["angle_info"],
+                          PLANE_SETTINGS["dist_info"], PLANE_SETTINGS["par_info"], PLANE_SETTINGS["ver_info"], PLANE_SETTINGS["plane_chi"], PLANE_SETTINGS["vp_chi"],
+                          0.05, 40, 1)
+    for k, v in kw.items():
+        setattr(p, k, v)
+    return p
+
+
+class PlanarTracker:
+    """PlanarSLAM's Tracking::Track() on the device (include/pslam_abi.h pslam_track_planar_*): Manhattan rotation, translation-only motion model, local map
+    with point, line and plane edges.  tracker = PlanarTracker(ctx); tracker.set_map(planar_map_dict) (synth_planar_map.build_planar_map shows the keys);
+    poses, Rcm, stats = tracker.track(gray [n,H,W] u8, depth [n,H,W] u16, Tcw0, vel0=None, Rcm0=None) - Rcm0 (mLastRcm before frame 0) defaults to
+    R_cw(Tcw0) * Rotation_cm, the Manhattan frame seen from the start pose."""
+
+    def __init__(self, ctx: Context, params: PlanarTrackParams | None = None):
+        self.ctx, self.params = ctx, params or default_planar_params(width=ctx.cfg.width, height=ctx.cfg.height)
+        L = ctx.L
+        L.pslam_track_set_planar_map.argtypes = [C.c_void_p, C.c_void_p]
+        L.pslam_track_planar_sequence.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p] + [C.c_void_p] * 6
+        self._keep, self.R_cm = None, None
+
+    def set_map(self, m: dict):
+        f32, f64, u8, i32 = np.float32, np.float64, np.uint8, np.int32
+        pt = {k: np.ascontiguousarray(m["points"][k], dt) for k, dt in (("pos", f32), ("normal", f32), ("max_distance", f32), ("min_distance", f32), ("desc", u8),
+                                                                         ("skip", u8), ("has_obs", u8))}
+        ln = {k: np.ascontiguousarray(m["lines"][k], dt) for k, dt in (("pos", f64), ("normal", f64), ("max_distance", f32), ("min_distance", f32), ("desc", u8),
+                                                                        ("skip", u8), ("has_obs", u8))}
+        pl = {k: np.ascontiguousarray(m["planes"][k], dt) for k, dt in (("coef", f32), ("bad", u8), ("pts_off", i32), ("pts", f32))}
+        ref = {k: np.ascontiguousarray(m[k], dt) for k, dt in (("ref_line_desc", u8), ("ref_line_map", i32))}
+        s = PlanarMapC()
+        s.points = MapPointsC(len(pt["skip"]), *[pt[k].ctypes.data for k in ("pos", "normal", "max_distance", "min_distance", "desc", "skip", "has_obs")])
+        s.lines = MapLinesC(len(ln["skip"]), *[ln[k].ctypes.data for k in ("pos", "normal", "max_distance", "min_distance", "desc", "skip", "has_obs")])
+        s.planes = MapPlanesC(len(pl["bad"]), *[pl[k].ctypes.data for k in ("coef", "bad", "pts_off", "pts")])
+        s.n_ref_lines, s.ref_line_desc, s.ref_line_map = len(ref["ref_line_map"]), ref["ref_line_desc"].ctypes.data, ref["ref_line_map"].ctypes.data
+        self.R_cm = np.ascontiguousarray(m["R_cm"], np.float32).reshape(3, 3)
+        s.R_cm[:] = [float(v) for v in self.R_cm.ravel()]
+        self._keep = (pt, ln, pl, ref)
+        self.ctx.check(self.ctx.L.pslam_track_set_planar_map(self.ctx.h, C.byref(s)))
+
+    def track(self, gray: np.ndarray, depth: np.ndarray, Tcw0: np.ndarray, vel0: np.ndarray | None = None, Rcm0: np.ndarray | None = None):
+        g, d = np.ascontiguousarray(gray, np.uint8), np.ascontiguousarray(depth, np.uint16)
+        n = len(g)
+        T0 = np.ascontiguousarray(Tcw0, np.float32)
+        v0 = None if vel0 is None else np.ascontiguousarray(vel0, np.float32)
+        if Rcm0 is None:
+            Rcm0 = (T0[:3, :3].astype(np.float64) @ self.R_cm.astype(np.float64)).astype(np.float32)
+        R0 = np.ascontiguousarray(Rcm0, np.float32)
+        poses, Rcm, stats = np.zeros((n, 4, 4), np.float32), np.zeros((n, 3, 3), np.float32), np.zeros((n, PLANAR_STATS), np.int32)
+        self.ctx.check(self.ctx.L.pslam_track_planar_sequence(self.ctx.h, g.ctypes.data, d.ctypes.data, n, C.byref(self.params), T0.ctypes.data,
+                                                              None if v0 is None else v0.ctypes.data, R0.ctypes.data, poses.ctypes.data, Rcm.ctypes.data,
+                                                              stats.ctypes.data))
+        return poses, Rcm, stats
