@@ -2,10 +2,11 @@
 // mvPlanePoints / mvPlaneCoefficients, and the surface normals (vSurfaceNormal) that TrackManhattanFrame consumes.  The three PCL algorithms behind those calls
 // are not in /root/reference; oracle/planepost.cc restates them (parity unpinned upstream, see its header) and the kernels here are held to that restatement.
 //
-//   k_planes_post    one CTA per (PEAC plane, frame): bounding box of the member points, voxel accumulation (leaf 0.1 m) into a shared-memory hash table with
-//                    ORDER-FREE 64-bit fixed-point sums (atomics), voxels sorted by index, the all-centroids-within-threshold test against the PEAC plane, PCL's
-//                    RANSAC (mt19937(12345) sample shuffling, <= 50 iterations, inlier counts by the whole CTA) and the float least-squares refit through the
-//                    closed-form eigen33, sign kept like the reference
+//   k_planes_worklist the (frame, plane) records of the planes PEAC found, plane-major
+//   k_planes_post    persistent CTAs (four per SM) that take one record at a time: voxel accumulation (leaf 0.1 m) into a shared-memory hash table with
+//                    ORDER-FREE fixed-point sums (32-bit atomics, see pp_base), the all-centroids-within-threshold test against the PEAC plane, occupied voxels
+//                    sorted by index, then on one warp PCL's RANSAC (mt19937(12345) sample shuffling, <= 50 iterations) and the float least-squares refit
+//                    through the closed-form eigen33, sign kept like the reference
 //   k_planes_compact one thread block per frame: the planes that survive, in PEAC order, with their voxel clouds packed
 //   k_sn_*           surface normals of the 3x sub-sampled organised cloud: points + depth-change map (parallel), the two chamfer passes (one warp per frame: the lanes
 //                    evaluate the terms from the neighbouring row, lane 0 walks the in-row chain of rounded additions), 3-D gradients + integral images in
@@ -25,13 +26,17 @@ namespace pslam {
 
 #define PP_SLOTS 2048            // occupied voxels per plane (a 20 m^2 plane at 0.1 m); more raise a status flag
 #define PP_THREADS 256
+#define PP_CTAS_PER_SM 4         // 48 KB of shared memory per CTA
+#define PP_SMEM ((size_t)PP_SLOTS * 6 * 4)
 #define PP_EMPTY 0xffffffffu
 #define PP_MAX_PLANES 128        // >= pslam_peac_max_planes()
+#define PP_MAX_PIXELS (1 << 25)  // members of one voxel: keeps the carry fields of the voxel sums below 2^10 (pp_base)
 
 struct PlanePostBuffers {
-    int max_batch = 0, maxp = 0, w3 = 0, h3 = 0;
+    int max_batch = 0, maxp = 0, w3 = 0, h3 = 0, workers = 0;
     // per (frame, plane) working records
     DevArray<float> d_coef; DevArray<int32_t> d_valid, d_npts; DevArray<float> d_pts; DevArray<int32_t> d_stats;     // [B][maxp][...]
+    DevArray<int32_t> d_work, d_ctl;                                                                                   // [B * maxp] records, [2] count / fetch counter
     // surface normals scratch
     DevArray<float> d_cloud, d_dist; DevArray<double> d_ix, d_iy;
     DevArray<float> d_nrm;
@@ -135,235 +140,349 @@ __device__ void pp_eigen33(const float m_in[3][3], float v[3]) {
     for (int k = 0; k < 3; ++k) v[k] = __fdiv_rn(best[k], len);
 }
 
-__global__ void __launch_bounds__(PP_THREADS) k_planes_post(const uint16_t* __restrict__ depth_all, int w, int h, PPCam K, const pslam_plane* __restrict__ planes_all,
-                                                            const int32_t* __restrict__ n_planes, const int32_t* __restrict__ midx_all,
-                                                            const int32_t* __restrict__ moff_all, int maxp, double dist_th, float* __restrict__ coef_out,
-                                                            int32_t* __restrict__ valid_out, int32_t* __restrict__ npts_out, float* __restrict__ pts_out,
-                                                            int32_t* __restrict__ stats_out, int32_t* __restrict__ status) {
-    extern __shared__ __align__(16) unsigned char pp_smem[];
-    unsigned long long* s_sum = reinterpret_cast<unsigned long long*>(pp_smem);                 // [3][PP_SLOTS]
-    uint32_t* s_key = reinterpret_cast<uint32_t*>(s_sum + 3 * PP_SLOTS);                          // [PP_SLOTS]
-    uint32_t* s_cnt = s_key + PP_SLOTS;                                                           // [PP_SLOTS]
-    float* s_px = reinterpret_cast<float*>(s_cnt + PP_SLOTS);                                     // [3][PP_SLOTS] sorted centroids
-    uint32_t* s_ord = reinterpret_cast<uint32_t*>(s_px + 3 * PP_SLOTS);                           // [PP_SLOTS] sort keys (voxel index << 11 | slot) / shuffled indices
-    uint32_t* s_mt = s_ord + PP_SLOTS;                                                            // [624]
-    __shared__ int s_i[8];
-    __shared__ float s_model[4];
-    const int pl = blockIdx.x, frame = blockIdx.y, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const size_t rec = (size_t)frame * maxp + pl;
-    if (pl >= min(n_planes[frame], maxp)) { if (tid == 0) { valid_out[rec] = 0; npts_out[rec] = 0; } return; }
-    const uint16_t* depth = depth_all + (size_t)frame * w * h;
-    const int32_t* moff = moff_all + (size_t)frame * (maxp + 1);
-    const int32_t* midx = midx_all + (size_t)frame * w * h + moff[pl];
-    const int nm = moff[pl + 1] - moff[pl];
-    for (int i = tid; i < PP_SLOTS; i += PP_THREADS) { s_key[i] = PP_EMPTY; s_cnt[i] = 0; s_sum[i] = 0; s_sum[PP_SLOTS + i] = 0; s_sum[2 * PP_SLOTS + i] = 0; }
-    for (int i = tid; i < 624; i += PP_THREADS) s_mt[i] = g_pp_mt[i];
-    if (tid == 0) { s_i[0] = 0; s_i[1] = 0; }
+// Exact, order-free voxel sums.  A member's coordinate enters as v = llrint(coordinate * 2^20); the sum of a voxel is kept relative to a base B(idx) of its
+// voxel index idx = floor(coordinate * 10) along that axis: every v - B lies in [0, 2^17) (v is within 26 units of [idx, idx + 1) * 104857.6 after the float
+// rounding of coordinate * 10, and idx is in [-512, 4094]), so a warp's group of at most 32 members sums to below 2^22 and enters the low 32-bit word of the
+// voxel with one atomicAdd.  Wraps of the low word are counted in a 10-bit field per axis of a shared carry word, which holds (sum >> 32) exactly while a voxel
+// has fewer than 2^25 members (PP_MAX_PIXELS).  The sums are integers, so the centroids do not depend on the order of the atomics.
+__device__ __forceinline__ int pp_base(int idx) { return idx * 104857 - 1024; }
+
+__device__ __forceinline__ float pp_centroid(uint32_t lo, uint32_t carries, uint32_t n, int idx, double n_fixed) {
+    const long long sum = (long long)(((unsigned long long)carries << 32) | lo) + (long long)n * pp_base(idx);
+    return (float)((double)sum / n_fixed);
+}
+
+// the (frame, plane) records of the planes PEAC found, plane-major: every frame's plane 0 comes first, and PEAC orders a frame's planes by size, so the largest
+// work is taken first and the launch ends on small planes.  ctl[0] = number of records, ctl[1] = the fetch counter of k_planes_post.  The order of the frames
+// within one plane index is that of the atomics; no output depends on it.
+__global__ void __launch_bounds__(1024) k_planes_worklist(int nframes, int maxp, const int32_t* __restrict__ n_planes, int32_t* __restrict__ work,
+                                                          int32_t* __restrict__ ctl) {
+    __shared__ int s_cnt[PP_MAX_PLANES], s_cur[PP_MAX_PLANES];
+    const int tid = threadIdx.x;
+    for (int p = tid; p < maxp; p += blockDim.x) s_cnt[p] = 0;
     __syncthreads();
-    // ---- voxel accumulation (leaf 0.1 m, order-free fixed-point sums) ----
-    // pcl::VoxelGrid numbers a voxel i0 + i1 * div0 + i2 * div0 * div1 with i* = floor(coordinate * 10) - floor(minimum * 10): ascending index = lexicographic
-    // (i2, i1, i0), which the packed absolute key (iz, iy, ix) below orders identically - so no bounding-box pass is needed.  The members of a plane are in pixel
-    // order and neighbouring pixels mostly share a voxel: every thread walks a contiguous run of members and only touches the table when the voxel changes.
-    const float inv = 10.0f;                                      // 1.0f / 0.1f rounds to 10.0f
-    {
-        const int chunk = (nm + PP_THREADS - 1) / PP_THREADS;
-        const int i_end = min(nm, (tid + 1) * chunk);
-        uint32_t run_key = PP_EMPTY, run_cnt = 0;
-        long long rx = 0, ry = 0, rz = 0;
-        auto flush = [&]() {
-            if (run_key == PP_EMPTY) return;
-            uint32_t slot = (run_key * 2654435761u) >> 21;         // 11 bits
-            bool placed = false;
-            for (int probe = 0; probe < PP_SLOTS; ++probe) {
-                const uint32_t cur = atomicCAS(&s_key[slot], PP_EMPTY, run_key);
-                if (cur == PP_EMPTY || cur == run_key) { placed = true; break; }
-                slot = (slot + 1) & (PP_SLOTS - 1);
-            }
-            if (!placed) { atomicOr(&s_i[1], 1); return; }
-            atomicAdd(&s_cnt[slot], run_cnt);
-            atomicAdd(&s_sum[slot], (unsigned long long)rx);
-            atomicAdd(&s_sum[PP_SLOTS + slot], (unsigned long long)ry);
-            atomicAdd(&s_sum[2 * PP_SLOTS + slot], (unsigned long long)rz);
-        };
-        // four members per trip: their index and depth loads are issued together (the walk was bound by the latency of one dependent load pair per member)
-        for (int ib = tid * chunk; ib < i_end; ib += 4) {
-          int pixv[4]; uint16_t dv[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) pixv[u] = ib + u < i_end ? midx[ib + u] : -1;
-#pragma unroll
-          for (int u = 0; u < 4; ++u) dv[u] = pixv[u] >= 0 ? depth[pixv[u]] : (uint16_t)0;
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            if (pixv[u] < 0) continue;
-            float x, y, z;
-            pp_vertex_d(dv[u], w, K, pixv[u], x, y, z);
-            const int i0 = (int)floorf(__fmul_rn(x, inv)) + 512, i1 = (int)floorf(__fmul_rn(y, inv)) + 512, i2 = (int)floorf(__fmul_rn(z, inv));
-            if ((unsigned)i0 > 1023u || (unsigned)i1 > 1023u || (unsigned)i2 >= 4095u) { atomicOr(&s_i[1], 1); continue; }      // > 51 m sideways / 409 m deep: capacity flag
-            const uint32_t key = ((uint32_t)i2 << 20) | ((uint32_t)i1 << 10) | (uint32_t)i0;
-            if (key != run_key) { flush(); run_key = key; run_cnt = 0; rx = ry = rz = 0; }
-            ++run_cnt;
-            rx += llrint((double)x * 1048576.0); ry += llrint((double)y * 1048576.0); rz += llrint((double)z * 1048576.0);
-          }
-        }
-        flush();
+    for (int f = tid; f < nframes; f += blockDim.x) {
+        const int n = min(n_planes[f], maxp);
+        for (int p = 0; p < n; ++p) atomicAdd(&s_cnt[p], 1);
     }
     __syncthreads();
-    // ---- order the occupied voxels by index: bitonic sort of (key, slot) pairs; empty slots sort last ----
-    // keys can exceed 21 bits, so the pair is sorted as 64-bit values held in two arrays: s_ord (slot) ordered by s_key through an index sort
-    for (int i = tid; i < PP_SLOTS; i += PP_THREADS) s_ord[i] = (uint32_t)i;
-    __syncthreads();
-    for (int size = 2; size <= PP_SLOTS; size <<= 1)
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int i = tid; i < PP_SLOTS / 2; i += PP_THREADS) {
-                const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
-                const bool up = ((lo & size) == 0);
-                const uint32_t a = s_ord[lo], b = s_ord[hi];
-                if ((s_key[a] > s_key[b]) == up) { s_ord[lo] = b; s_ord[hi] = a; }
-            }
-            __syncthreads();
-        }
-    if (tid == 0) { int n = 0; while (n < PP_SLOTS && s_key[s_ord[n]] != PP_EMPTY) ++n; s_i[0] = n; }
-    __syncthreads();
-    const int N = s_i[0];
-    for (int i = tid; i < N; i += PP_THREADS) {
-        const uint32_t sl = s_ord[i];
-        const double n = (double)s_cnt[sl] * 1048576.0;
-        s_px[i] = (float)((double)(long long)s_sum[sl] / n);
-        s_px[PP_SLOTS + i] = (float)((double)(long long)s_sum[PP_SLOTS + sl] / n);
-        s_px[2 * PP_SLOTS + i] = (float)((double)(long long)s_sum[2 * PP_SLOTS + sl] / n);
+    if (tid == 0) {
+        int off = 0;
+        for (int p = 0; p < maxp; ++p) { s_cur[p] = off; off += s_cnt[p]; }
+        ctl[0] = off; ctl[1] = 0;
     }
     __syncthreads();
-    // ---- MaxPointDistanceFromPlane: every centroid within the threshold of the PEAC plane ----
-    const pslam_plane P = planes_all[rec];
-    float coef[4] = {(float)P.normal[0], (float)P.normal[1], (float)P.normal[2],
-                     (float)-(P.normal[0] * P.center[0] + P.normal[1] * P.center[1] + P.normal[2] * P.center[2])};
-    int bad = 0;
-    for (int i = tid; i < N; i += PP_THREADS) bad |= (double)fabsf(pp_dot4(coef, s_px[i], s_px[PP_SLOTS + i], s_px[2 * PP_SLOTS + i])) > dist_th;
-    bad = __syncthreads_or(bad);
-    if (bad || N < 3) { if (tid == 0) { valid_out[rec] = 0; npts_out[rec] = 0; stats_out[2 * rec] = 0; stats_out[2 * rec + 1] = 0; if (s_i[1]) atomicOr(status + frame, 32); } return; }
-    // ---- RANSAC (pcl::RandomSampleConsensus on SampleConsensusModelPlane) ----
-    uint32_t* shuffled = s_ord;                                   // the sort order is no longer needed
-    for (int i = tid; i < N; i += PP_THREADS) shuffled[i] = (uint32_t)i;
-    PPRng rng; rng.mt = s_mt; rng.idx = 0;                       // s_mt: mt19937(12345) after its first twist (copied from g_pp_mt above)
-    __syncthreads();
-    int best_count = -INT_MAX, iterations = 0;
-    double k = 1.0;
-    const double log_probability = log(1.0 - 0.99), one_over = 1.0 / (double)N;
-    float best[4] = {0, 0, 0, 0};
-    bool have = false;
-    unsigned skipped = 0;
-    while (iterations < k && skipped < 500u) {
-        if (tid == 0) {
-            int s0 = 0, s1 = 0, s2 = 0;
-            bool good = false;
-            for (unsigned it = 0; it < 1000 && !good; ++it) {
-                for (int i = 0; i < 3; ++i) { const int j = i + (rng.rnd() % (N - i)); const uint32_t t = shuffled[i]; shuffled[i] = shuffled[j]; shuffled[j] = t; }
-                s0 = shuffled[0]; s1 = shuffled[1]; s2 = shuffled[2];
-                const float d0 = __fdiv_rn(__fsub_rn(s_px[s1], s_px[s0]), __fsub_rn(s_px[s2], s_px[s0]));
-                const float d1 = __fdiv_rn(__fsub_rn(s_px[PP_SLOTS + s1], s_px[PP_SLOTS + s0]), __fsub_rn(s_px[PP_SLOTS + s2], s_px[PP_SLOTS + s0]));
-                const float d2 = __fdiv_rn(__fsub_rn(s_px[2 * PP_SLOTS + s1], s_px[2 * PP_SLOTS + s0]), __fsub_rn(s_px[2 * PP_SLOTS + s2], s_px[2 * PP_SLOTS + s0]));
-                good = (d0 != d1) || (d2 != d1);
-            }
-            int state = good ? 1 : 0;                             // 0: no sample, 1: model, 2: degenerate (skipped)
-            if (good) {
-                const float a[3] = {__fsub_rn(s_px[s1], s_px[s0]), __fsub_rn(s_px[PP_SLOTS + s1], s_px[PP_SLOTS + s0]), __fsub_rn(s_px[2 * PP_SLOTS + s1], s_px[2 * PP_SLOTS + s0])};
-                const float b[3] = {__fsub_rn(s_px[s2], s_px[s0]), __fsub_rn(s_px[PP_SLOTS + s2], s_px[PP_SLOTS + s0]), __fsub_rn(s_px[2 * PP_SLOTS + s2], s_px[2 * PP_SLOTS + s0])};
-                const float e0 = __fdiv_rn(a[0], b[0]), e1 = __fdiv_rn(a[1], b[1]), e2 = __fdiv_rn(a[2], b[2]);
-                if (e0 == e1 && e2 == e1) state = 2;
-                else {
-                    float c[3] = {__fsub_rn(__fmul_rn(a[1], b[2]), __fmul_rn(a[2], b[1])), __fsub_rn(__fmul_rn(a[2], b[0]), __fmul_rn(a[0], b[2])),
-                                  __fsub_rn(__fmul_rn(a[0], b[1]), __fmul_rn(a[1], b[0]))};
-                    const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(c[0], c[0]), __fmul_rn(c[1], c[1])), __fmul_rn(c[2], c[2])));
-                    for (int q = 0; q < 3; ++q) c[q] = __fdiv_rn(c[q], nrm);
-                    s_model[0] = c[0]; s_model[1] = c[1]; s_model[2] = c[2];
-                    s_model[3] = -1 * __fadd_rn(__fadd_rn(__fmul_rn(c[0], s_px[s0]), __fmul_rn(c[1], s_px[PP_SLOTS + s0])), __fmul_rn(c[2], s_px[2 * PP_SLOTS + s0]));
+    for (int f = tid; f < nframes; f += blockDim.x) {
+        const int n = min(n_planes[f], maxp);
+        for (int p = 0; p < n; ++p) work[atomicAdd(&s_cur[p], 1)] = f * maxp + p;
+    }
+}
+
+// one group of members that share a voxel: probe for its slot, then add the count and the three relative sums (leader lane only)
+__device__ __forceinline__ void pp_voxel_add(uint32_t* s_key, uint32_t* s_cnt, uint32_t* s_carry, uint32_t* s_lo, uint32_t key, uint32_t n, uint32_t sx,
+                                             uint32_t sy, uint32_t sz, int* flag) {
+    uint32_t slot = (key * 2654435761u) >> 21;                    // 11 bits
+    bool placed = false;
+    for (int probe = 0; probe < PP_SLOTS; ++probe) {
+        const uint32_t cur = atomicCAS(&s_key[slot], PP_EMPTY, key);
+        if (cur == PP_EMPTY || cur == key) { placed = true; break; }
+        slot = (slot + 1) & (PP_SLOTS - 1);
+    }
+    if (!placed) { atomicOr(flag, 1); return; }
+    atomicAdd(&s_cnt[slot], n);
+    const uint32_t d[3] = {sx, sy, sz};
+    uint32_t carry = 0;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        const uint32_t old = atomicAdd(&s_lo[a * PP_SLOTS + slot], d[a]);
+        if (old + d[a] < old) carry += 1u << (10 * a);
+    }
+    if (carry) atomicAdd(&s_carry[slot], carry);
+}
+
+__global__ void __launch_bounds__(PP_THREADS, PP_CTAS_PER_SM) k_planes_post(const uint16_t* __restrict__ depth_all, int w, int h, PPCam K,
+                                                                            const pslam_plane* __restrict__ planes_all, const int32_t* __restrict__ work,
+                                                                            int32_t* __restrict__ ctl, const int32_t* __restrict__ midx_all,
+                                                                            const int32_t* __restrict__ moff_all, int maxp, double dist_th, float* __restrict__ coef_out,
+                                                                            int32_t* __restrict__ valid_out, int32_t* __restrict__ npts_out, float* __restrict__ pts_out,
+                                                                            int32_t* __restrict__ stats_out, int32_t* __restrict__ status) {
+    constexpr int PER_THREAD = PP_SLOTS / PP_THREADS;
+    constexpr uint32_t FULL = 0xffffffffu;
+    extern __shared__ __align__(16) uint32_t pp_smem[];
+    // 48 KB, reused from phase to phase: voxel table -> centroids by slot + sort order -> sorted centroids + RANSAC state
+    uint32_t* s_key = pp_smem;                     // [PP_SLOTS] voxel keys; then sorted x
+    uint32_t* s_cnt = s_key + PP_SLOTS;            // [PP_SLOTS] member counts; then the sort order; then the mt19937 state
+    uint32_t* s_carry = s_cnt + PP_SLOTS;          // [PP_SLOTS] carry fields of the sums; then sorted y
+    uint32_t* s_lo = s_carry + PP_SLOTS;           // [3][PP_SLOTS] low words of the sums; then the centroids by slot; then sorted z, shuffled indices, inlier list
+    float* s_px = reinterpret_cast<float*>(s_lo);
+    __shared__ int s_i[4];                         // occupied voxels, capacity flag, record
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const float inv = 10.0f;                       // 1.0f / 0.1f rounds to 10.0f
+    for (;;) {
+        __syncthreads();                           // the previous record's shared memory is no longer read
+        if (tid == 0) { s_i[0] = 0; s_i[1] = 0; const int item = atomicAdd(ctl + 1, 1); s_i[2] = item < ctl[0] ? item : -1; }
+        {
+            uint4* t = reinterpret_cast<uint4*>(pp_smem);
+            for (int i = tid; i < PP_SLOTS / 4; i += PP_THREADS) t[i] = make_uint4(PP_EMPTY, PP_EMPTY, PP_EMPTY, PP_EMPTY);
+            for (int i = PP_SLOTS / 4 + tid; i < 6 * PP_SLOTS / 4; i += PP_THREADS) t[i] = make_uint4(0, 0, 0, 0);
+        }
+        __syncthreads();
+        const int item = s_i[2];
+        if (item < 0) return;
+        const int rec = work[item], frame = rec / maxp, pl = rec - frame * maxp;
+        const uint16_t* depth = depth_all + (size_t)frame * w * h;
+        const int32_t* moff = moff_all + (size_t)frame * (maxp + 1);
+        const int32_t* midx = midx_all + (size_t)frame * w * h + moff[pl];
+        const int nm = moff[pl + 1] - moff[pl];
+        // ---- voxel accumulation (leaf 0.1 m) ----
+        // pcl::VoxelGrid numbers a voxel i0 + i1 * div0 + i2 * div0 * div1 with i* = floor(coordinate * 10) - floor(minimum * 10): ascending index = lexicographic
+        // (i2, i1, i0), which the packed absolute key (iz, iy, ix) below orders identically - so no bounding-box pass is needed.  A warp reads 4 x 32 consecutive
+        // members per trip (their index loads, then their depth loads, issued together); lanes of one trip that share a voxel are grouped by __match_any_sync and
+        // their sums reduced, so the table sees one update per distinct voxel and trip.
+        for (int base = wid * 128; base < nm; base += PP_THREADS * 4) {
+            int pix[4]; uint16_t dv[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) { const int i = base + 32 * u + lane; pix[u] = i < nm ? midx[i] : -1; }
+#pragma unroll
+            for (int u = 0; u < 4; ++u) dv[u] = pix[u] >= 0 ? depth[pix[u]] : (uint16_t)0;
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                if (base + 32 * u >= nm) break;
+                uint32_t key = PP_EMPTY, dx = 0, dy = 0, dz = 0;
+                if (pix[u] >= 0) {
+                    float x, y, z;
+                    pp_vertex_d(dv[u], w, K, pix[u], x, y, z);
+                    const int j0 = (int)floorf(__fmul_rn(x, inv)), j1 = (int)floorf(__fmul_rn(y, inv)), j2 = (int)floorf(__fmul_rn(z, inv));
+                    const int i0 = j0 + 512, i1 = j1 + 512, i2 = j2;
+                    if ((unsigned)i0 > 1023u || (unsigned)i1 > 1023u || (unsigned)i2 >= 4095u) atomicOr(&s_i[1], 1);      // > 51 m sideways / 409 m deep: capacity flag
+                    else {
+                        key = ((uint32_t)i2 << 20) | ((uint32_t)i1 << 10) | (uint32_t)i0;
+                        // llrint((double)x * 2^20): the scaling is exact in float as well, and |v| < 2^29 inside the key range
+                        dx = (uint32_t)(__float2int_rn(__fmul_rn(x, 1048576.0f)) - pp_base(j0));
+                        dy = (uint32_t)(__float2int_rn(__fmul_rn(y, 1048576.0f)) - pp_base(j1));
+                        dz = (uint32_t)(__float2int_rn(__fmul_rn(z, 1048576.0f)) - pp_base(j2));
+                    }
+                }
+                const uint32_t grp = __match_any_sync(FULL, key);
+                uint32_t leaders = __ballot_sync(FULL, key != PP_EMPTY && (grp & ((1u << lane) - 1u)) == 0);
+                while (leaders) {
+                    const int ld = __ffs(leaders) - 1;
+                    leaders &= leaders - 1;
+                    const uint32_t g = __shfl_sync(FULL, grp, ld);
+                    const bool in = (g >> lane) & 1u;
+                    const uint32_t sx = __reduce_add_sync(FULL, in ? dx : 0u), sy = __reduce_add_sync(FULL, in ? dy : 0u), sz = __reduce_add_sync(FULL, in ? dz : 0u);
+                    if (lane == ld) pp_voxel_add(s_key, s_cnt, s_carry, s_lo, key, __popc(g), sx, sy, sz, &s_i[1]);
                 }
             }
-            s_i[2] = state; s_i[3] = 0;
         }
         __syncthreads();
-        const int state = s_i[2];
-        if (state == 0) break;
-        if (state == 2) { ++skipped; __syncthreads(); continue; }
-        const float c[4] = {s_model[0], s_model[1], s_model[2], s_model[3]};
-        int cnt = 0;
-        for (int i = tid; i < N; i += PP_THREADS) cnt += (double)fabsf(pp_dot4(c, s_px[i], s_px[PP_SLOTS + i], s_px[2 * PP_SLOTS + i])) < dist_th;
-        for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-        if (lane == 0) atomicAdd(&s_i[3], cnt);
-        __syncthreads();
-        cnt = s_i[3];
-        if (cnt > best_count) {
-            best_count = cnt; best[0] = c[0]; best[1] = c[1]; best[2] = c[2]; best[3] = c[3]; have = true;
-            const double wv = (double)best_count * one_over;
-            double p_no = 1.0 - pow(wv, 3.0);
-            p_no = fmax(DBL_EPSILON, p_no);
-            p_no = fmin(1.0 - DBL_EPSILON, p_no);
-            k = log_probability / log(p_no);
+        // ---- centroids (each thread overwrites the sums of its own slots) and MaxPointDistanceFromPlane: every centroid within the threshold of the PEAC plane ----
+        const pslam_plane P = planes_all[rec];
+        const float coef[4] = {(float)P.normal[0], (float)P.normal[1], (float)P.normal[2],
+                               (float)-(P.normal[0] * P.center[0] + P.normal[1] * P.center[1] + P.normal[2] * P.center[2])};
+        int bad = 0;
+        for (int s = tid; s < PP_SLOTS; s += PP_THREADS) {
+            const uint32_t key = s_key[s];
+            if (key == PP_EMPTY) continue;
+            const uint32_t n = s_cnt[s], carries = s_carry[s];
+            const double n_fixed = (double)n * 1048576.0;
+            const float x = pp_centroid(s_lo[s], carries & 1023u, n, (int)(key & 1023u) - 512, n_fixed);
+            const float y = pp_centroid(s_lo[PP_SLOTS + s], (carries >> 10) & 1023u, n, (int)((key >> 10) & 1023u) - 512, n_fixed);
+            const float z = pp_centroid(s_lo[2 * PP_SLOTS + s], carries >> 20, n, (int)(key >> 20), n_fixed);
+            s_px[s] = x; s_px[PP_SLOTS + s] = y; s_px[2 * PP_SLOTS + s] = z;
+            bad |= (double)fabsf(pp_dot4(coef, x, y, z)) > dist_th;
         }
-        ++iterations;
+        bad = __syncthreads_or(bad);
+        uint32_t* s_ord = s_cnt;
+        int N = 0;
+        if (!bad) {                                // the occupied slots, compacted
+            for (int s = tid; s < PP_SLOTS; s += PP_THREADS) {
+                const bool o = s_key[s] != PP_EMPTY;
+                const uint32_t m = __ballot_sync(FULL, o);
+                int at = 0;
+                if (lane == 0 && m) at = atomicAdd(&s_i[0], __popc(m));
+                at = __shfl_sync(FULL, at, 0);
+                if (o) s_ord[at + __popc(m & ((1u << lane) - 1u))] = (uint32_t)s;
+            }
+            __syncthreads();
+            N = s_i[0];
+        }
+        if (bad || N < 3) {
+            if (tid == 0) { valid_out[rec] = 0; npts_out[rec] = 0; stats_out[2 * rec] = 0; stats_out[2 * rec + 1] = 0; if (s_i[1]) atomicOr(status + frame, 32); }
+            continue;
+        }
+        // ---- order the occupied voxels by index: bitonic sort of their slots by key over the next power of two (keys are unique, pads sort last) ----
+        int n2 = 4;
+        while (n2 < N) n2 <<= 1;
+        for (int i = N + tid; i < n2; i += PP_THREADS) s_ord[i] = PP_EMPTY;
         __syncthreads();
-        if (iterations > 50) break;
-    }
-    if (!have) { if (tid == 0) { valid_out[rec] = 0; npts_out[rec] = 0; stats_out[2 * rec] = 0; stats_out[2 * rec + 1] = iterations; } return; }
-    // ---- optimizeModelCoefficients (thread 0: sequential float moments in index order) + selectWithinDistance with the refined model ----
-    if (tid == 0) {
-        float acc[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        for (int size = 2; size <= n2; size <<= 1)
+            for (int stride = size >> 1; stride > 0; stride >>= 1) {
+                for (int i = tid; i < n2 / 2; i += PP_THREADS) {
+                    const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
+                    const bool up = ((lo & size) == 0);
+                    const uint32_t a = s_ord[lo], b = s_ord[hi];
+                    const uint32_t ka = a == PP_EMPTY ? PP_EMPTY : s_key[a], kb = b == PP_EMPTY ? PP_EMPTY : s_key[b];
+                    if ((ka > kb) == up) { s_ord[lo] = b; s_ord[hi] = a; }
+                }
+                __syncthreads();
+            }
+        // sorted centroids: x over the keys, y over the carries, z (through registers) over the slot-order x
+        float* px = reinterpret_cast<float*>(s_key);
+        float* py = reinterpret_cast<float*>(s_carry);
+        float* pz = s_px;
+        float zk[PER_THREAD];
+#pragma unroll
+        for (int k = 0; k < PER_THREAD; ++k) {
+            const int i = tid + k * PP_THREADS;
+            zk[k] = 0.f;
+            if (i < N) { const uint32_t o = s_ord[i]; px[i] = s_px[o]; py[i] = s_px[PP_SLOTS + o]; zk[k] = s_px[2 * PP_SLOTS + o]; }
+        }
+        __syncthreads();
+        uint32_t* shuffled = s_lo + PP_SLOTS;
+        uint32_t* s_inl = s_lo + 2 * PP_SLOTS;
+#pragma unroll
+        for (int k = 0; k < PER_THREAD; ++k) {
+            const int i = tid + k * PP_THREADS;
+            if (i < N) { pz[i] = zk[k]; shuffled[i] = (uint32_t)i; }
+        }
+        for (int i = tid; i < 624; i += PP_THREADS) s_cnt[i] = g_pp_mt[i];      // mt19937(12345) after its first twist
+        __syncthreads();
+        if (wid != 0) continue;
+        // ---- RANSAC (pcl::RandomSampleConsensus on SampleConsensusModelPlane) on warp 0: lane 0 draws the samples in the reference's order, the lanes count ----
+        PPRng rng; rng.mt = s_cnt; rng.idx = 0;
+        int best_count = -INT_MAX, iterations = 0;
+        double k = 1.0;
+        const double log_probability = log(1.0 - 0.99), one_over = 1.0 / (double)N;
+        float best[4] = {0, 0, 0, 0};
+        bool have = false;
+        unsigned skipped = 0;
+        while (iterations < k && skipped < 500u) {
+            int state = 0;                                            // 0: no sample, 1: model, 2: degenerate (skipped)
+            float c[4] = {0, 0, 0, 0};
+            if (lane == 0) {
+                int s0 = 0, s1 = 0, s2 = 0;
+                bool good = false;
+                for (unsigned it = 0; it < 1000 && !good; ++it) {
+                    for (int i = 0; i < 3; ++i) { const int j = i + (rng.rnd() % (N - i)); const uint32_t t = shuffled[i]; shuffled[i] = shuffled[j]; shuffled[j] = t; }
+                    s0 = shuffled[0]; s1 = shuffled[1]; s2 = shuffled[2];
+                    const float d0 = __fdiv_rn(__fsub_rn(px[s1], px[s0]), __fsub_rn(px[s2], px[s0]));
+                    const float d1 = __fdiv_rn(__fsub_rn(py[s1], py[s0]), __fsub_rn(py[s2], py[s0]));
+                    const float d2 = __fdiv_rn(__fsub_rn(pz[s1], pz[s0]), __fsub_rn(pz[s2], pz[s0]));
+                    good = (d0 != d1) || (d2 != d1);
+                }
+                state = good ? 1 : 0;
+                if (good) {
+                    const float a[3] = {__fsub_rn(px[s1], px[s0]), __fsub_rn(py[s1], py[s0]), __fsub_rn(pz[s1], pz[s0])};
+                    const float b[3] = {__fsub_rn(px[s2], px[s0]), __fsub_rn(py[s2], py[s0]), __fsub_rn(pz[s2], pz[s0])};
+                    const float e0 = __fdiv_rn(a[0], b[0]), e1 = __fdiv_rn(a[1], b[1]), e2 = __fdiv_rn(a[2], b[2]);
+                    if (e0 == e1 && e2 == e1) state = 2;
+                    else {
+                        c[0] = __fsub_rn(__fmul_rn(a[1], b[2]), __fmul_rn(a[2], b[1]));
+                        c[1] = __fsub_rn(__fmul_rn(a[2], b[0]), __fmul_rn(a[0], b[2]));
+                        c[2] = __fsub_rn(__fmul_rn(a[0], b[1]), __fmul_rn(a[1], b[0]));
+                        const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(c[0], c[0]), __fmul_rn(c[1], c[1])), __fmul_rn(c[2], c[2])));
+                        for (int q = 0; q < 3; ++q) c[q] = __fdiv_rn(c[q], nrm);
+                        c[3] = -1 * __fadd_rn(__fadd_rn(__fmul_rn(c[0], px[s0]), __fmul_rn(c[1], py[s0])), __fmul_rn(c[2], pz[s0]));
+                    }
+                }
+            }
+            state = __shfl_sync(FULL, state, 0);
+            if (state == 0) break;
+            if (state == 2) { ++skipped; continue; }
+#pragma unroll
+            for (int q = 0; q < 4; ++q) c[q] = __shfl_sync(FULL, c[q], 0);
+            unsigned cnt = 0;
+            for (int i = lane; i < N; i += 32) cnt += (double)fabsf(pp_dot4(c, px[i], py[i], pz[i])) < dist_th;
+            const int total = (int)__reduce_add_sync(FULL, cnt);
+            if (total > best_count) {
+                best_count = total; best[0] = c[0]; best[1] = c[1]; best[2] = c[2]; best[3] = c[3]; have = true;
+                if (lane == 0) {
+                    const double wv = (double)best_count * one_over;
+                    double p_no = 1.0 - pow(wv, 3.0);
+                    p_no = fmax(DBL_EPSILON, p_no);
+                    p_no = fmin(1.0 - DBL_EPSILON, p_no);
+                    k = log_probability / log(p_no);
+                }
+                k = __shfl_sync(FULL, k, 0);
+            }
+            ++iterations;
+            if (iterations > 50) break;
+        }
+        if (!have) {
+            if (lane == 0) { valid_out[rec] = 0; npts_out[rec] = 0; stats_out[2 * rec] = 0; stats_out[2 * rec + 1] = iterations; }
+            continue;
+        }
+        // ---- optimizeModelCoefficients: the inliers of the best model listed in index order, then nine lanes walk one float moment each in that order (the
+        //      sequential loop's chains of rounded additions, term by term; the first-order terms are x * 1.0f = x) ----
         int ninl = 0;
-        for (int i = 0; i < N; ++i) {
-            const float x = s_px[i], y = s_px[PP_SLOTS + i], z = s_px[2 * PP_SLOTS + i];
-            if (!((double)fabsf(pp_dot4(best, x, y, z)) < dist_th)) continue;
-            ++ninl;
-            acc[0] = __fadd_rn(acc[0], __fmul_rn(x, x)); acc[1] = __fadd_rn(acc[1], __fmul_rn(x, y)); acc[2] = __fadd_rn(acc[2], __fmul_rn(x, z));
-            acc[3] = __fadd_rn(acc[3], __fmul_rn(y, y)); acc[4] = __fadd_rn(acc[4], __fmul_rn(y, z)); acc[5] = __fadd_rn(acc[5], __fmul_rn(z, z));
-            acc[6] = __fadd_rn(acc[6], x); acc[7] = __fadd_rn(acc[7], y); acc[8] = __fadd_rn(acc[8], z);
+        for (int b = 0; b < N; b += 32) {
+            const int i = b + lane;
+            const bool in = i < N && (double)fabsf(pp_dot4(best, px[i], py[i], pz[i])) < dist_th;
+            const uint32_t m = __ballot_sync(FULL, in);
+            if (in) s_inl[ninl + __popc(m & ((1u << lane) - 1u))] = (uint32_t)i;
+            ninl += __popc(m);
         }
+        __syncwarp();
+        float acc = 0.f;
+        if (lane < 9) {
+            const int ua = lane < 3 ? 0 : lane < 5 ? 1 : lane < 6 ? 2 : -1;
+            const int vb = lane < 6 ? (lane < 3 ? lane : lane < 5 ? lane - 2 : 2) : lane - 6;
+            const float* pu = ua == 1 ? py : ua == 2 ? pz : px;
+            const float* pv = vb == 0 ? px : vb == 1 ? py : pz;
+#pragma unroll 4
+            for (int t = 0; t < ninl; ++t) {
+                const uint32_t i = s_inl[t];
+                const float u = ua < 0 ? 1.0f : pu[i];
+                acc = __fadd_rn(acc, __fmul_rn(u, pv[i]));
+            }
+        }
+        float m9[9];
+#pragma unroll
+        for (int q = 0; q < 9; ++q) m9[q] = __shfl_sync(FULL, acc, q);
         float opt[4] = {best[0], best[1], best[2], best[3]};
         if (ninl > 3) {
-            for (int q = 0; q < 9; ++q) acc[q] = __fdiv_rn(acc[q], (float)ninl);
+            for (int q = 0; q < 9; ++q) m9[q] = __fdiv_rn(m9[q], (float)ninl);
             float cov[3][3];
-            cov[0][0] = __fsub_rn(acc[0], __fmul_rn(acc[6], acc[6])); cov[0][1] = __fsub_rn(acc[1], __fmul_rn(acc[6], acc[7])); cov[0][2] = __fsub_rn(acc[2], __fmul_rn(acc[6], acc[8]));
-            cov[1][1] = __fsub_rn(acc[3], __fmul_rn(acc[7], acc[7])); cov[1][2] = __fsub_rn(acc[4], __fmul_rn(acc[7], acc[8])); cov[2][2] = __fsub_rn(acc[5], __fmul_rn(acc[8], acc[8]));
+            cov[0][0] = __fsub_rn(m9[0], __fmul_rn(m9[6], m9[6])); cov[0][1] = __fsub_rn(m9[1], __fmul_rn(m9[6], m9[7])); cov[0][2] = __fsub_rn(m9[2], __fmul_rn(m9[6], m9[8]));
+            cov[1][1] = __fsub_rn(m9[3], __fmul_rn(m9[7], m9[7])); cov[1][2] = __fsub_rn(m9[4], __fmul_rn(m9[7], m9[8])); cov[2][2] = __fsub_rn(m9[5], __fmul_rn(m9[8], m9[8]));
             cov[1][0] = cov[0][1]; cov[2][0] = cov[0][2]; cov[2][1] = cov[1][2];
             float vec[3];
             pp_eigen33(cov, vec);
             opt[0] = vec[0]; opt[1] = vec[1]; opt[2] = vec[2];
-            opt[3] = -1 * __fadd_rn(__fadd_rn(__fmul_rn(opt[0], acc[6]), __fmul_rn(opt[1], acc[7])), __fmul_rn(opt[2], acc[8]));
+            opt[3] = -1 * __fadd_rn(__fadd_rn(__fmul_rn(opt[0], m9[6]), __fmul_rn(opt[1], m9[7])), __fmul_rn(opt[2], m9[8]));
         }
-        s_model[0] = opt[0]; s_model[1] = opt[1]; s_model[2] = opt[2]; s_model[3] = opt[3];
-        s_i[3] = 0; s_i[4] = ninl;
+        // ---- selectWithinDistance with the refined model ----
+        unsigned cnt = 0;
+        for (int i = lane; i < N; i += 32) cnt += (double)fabsf(pp_dot4(opt, px[i], py[i], pz[i])) < dist_th;
+        const int final_inl = (int)__reduce_add_sync(FULL, cnt);
+        if (final_inl == 0 || ninl == 0) {
+            if (lane == 0) { valid_out[rec] = 0; npts_out[rec] = 0; }
+            continue;
+        }
+        const float old_d = coef[3], new_d = opt[3];
+        if ((new_d < 0 && old_d > 0) || (new_d > 0 && old_d < 0)) for (int q = 0; q < 4; ++q) opt[q] = -opt[q];
+        if (lane == 0) {
+            for (int q = 0; q < 4; ++q) coef_out[(size_t)rec * 4 + q] = opt[q];
+            valid_out[rec] = 1; npts_out[rec] = N; stats_out[2 * rec] = final_inl; stats_out[2 * rec + 1] = iterations;
+            if (s_i[1]) atomicOr(status + frame, 32);
+        }
+        float* po = pts_out + (size_t)rec * PP_SLOTS * 3;
+        for (int i = lane; i < 3 * N; i += 32) { const int v = i / 3, q = i - 3 * v; po[i] = (q == 0 ? px : q == 1 ? py : pz)[v]; }
     }
-    __syncthreads();
-    {
-        const float c[4] = {s_model[0], s_model[1], s_model[2], s_model[3]};
-        int cnt = 0;
-        for (int i = tid; i < N; i += PP_THREADS) cnt += (double)fabsf(pp_dot4(c, s_px[i], s_px[PP_SLOTS + i], s_px[2 * PP_SLOTS + i])) < dist_th;
-        for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-        if (lane == 0) atomicAdd(&s_i[3], cnt);
-    }
-    __syncthreads();
-    const int final_inl = s_i[3];
-    if (final_inl == 0 || s_i[4] == 0) { if (tid == 0) { valid_out[rec] = 0; npts_out[rec] = 0; } return; }
-    float outc[4] = {s_model[0], s_model[1], s_model[2], s_model[3]};
-    const float old_d = coef[3], new_d = outc[3];
-    if ((new_d < 0 && old_d > 0) || (new_d > 0 && old_d < 0)) for (int q = 0; q < 4; ++q) outc[q] = -outc[q];
-    if (tid == 0) {
-        for (int q = 0; q < 4; ++q) coef_out[rec * 4 + q] = outc[q];
-        valid_out[rec] = 1; npts_out[rec] = N; stats_out[2 * rec] = final_inl; stats_out[2 * rec + 1] = iterations;
-        if (s_i[1]) atomicOr(status + frame, 32);
-    }
-    float* po = pts_out + rec * (size_t)PP_SLOTS * 3;
-    for (int i = tid; i < N; i += PP_THREADS) { po[3 * i] = s_px[i]; po[3 * i + 1] = s_px[PP_SLOTS + i]; po[3 * i + 2] = s_px[2 * PP_SLOTS + i]; }
 }
 
 // the surviving planes of a frame, in PEAC order: src [maxp], coef [maxp][4], pt_off [maxp + 1], pts packed
-__global__ void __launch_bounds__(256) k_planes_compact(int maxp, int cap_pts, const float* __restrict__ coef_w, const int32_t* __restrict__ valid_w, const int32_t* __restrict__ npts_w,
-                                                        const float* __restrict__ pts_w, int32_t* __restrict__ n_kept, int32_t* __restrict__ src, float* __restrict__ coef,
-                                                        int32_t* __restrict__ pt_off, float* __restrict__ pts, int32_t* __restrict__ status) {
+__global__ void __launch_bounds__(256) k_planes_compact(int maxp, int cap_pts, const int32_t* __restrict__ n_planes, const float* __restrict__ coef_w,
+                                                        const int32_t* __restrict__ valid_w, const int32_t* __restrict__ npts_w, const float* __restrict__ pts_w,
+                                                        int32_t* __restrict__ n_kept, int32_t* __restrict__ src, float* __restrict__ coef, int32_t* __restrict__ pt_off,
+                                                        float* __restrict__ pts, int32_t* __restrict__ status) {
     const int frame = blockIdx.x, tid = threadIdx.x;
     __shared__ int s_slot[PP_MAX_PLANES], s_off[PP_MAX_PLANES + 1], s_n;
     if (tid == 0) {
         int n = 0, off = 0;
-        for (int p = 0; p < maxp; ++p) {
+        const int np = min(n_planes[frame], maxp);                // records past n_planes are not written by k_planes_post
+        for (int p = 0; p < np; ++p) {
             const size_t rec = (size_t)frame * maxp + p;
             if (!valid_w[rec]) continue;
             s_slot[n] = p; s_off[n] = off; off += npts_w[rec]; ++n;
@@ -584,7 +703,19 @@ static int planepost_alloc(pslam_ctx* c) {
     c->planepost = Bp;
     B.max_batch = c->cfg.max_batch; B.maxp = pslam_peac_max_planes(c);
     if (B.maxp > PP_MAX_PLANES) { planepost_free(c); return set_error(c, PSLAM_E_INVALID, "plane capacity above the post-processing limit"); }
+    if ((size_t)c->cfg.width * c->cfg.height > (size_t)PP_MAX_PIXELS) { planepost_free(c); return set_error(c, PSLAM_E_INVALID, "image above the plane post-processing limit"); }
     B.w3 = (c->cfg.width + 2) / 3; B.h3 = (c->cfg.height + 2) / 3;
+    {   // the persistent grid of k_planes_post: as many CTAs as are resident at once
+        int sms = 0, per_sm = 0;
+        int rc_ = check_cuda(c, cudaFuncSetAttribute(k_planes_post, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PP_SMEM), "cudaFuncSetAttribute(k_planes_post)");
+        if (rc_ == PSLAM_OK) rc_ = check_cuda(c, cudaFuncSetAttribute(k_planes_post, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared),
+                                              "cudaFuncSetAttribute(k_planes_post)");
+        if (rc_ == PSLAM_OK) rc_ = check_cuda(c, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->cfg.device), "cudaDeviceGetAttribute");
+        if (rc_ == PSLAM_OK) rc_ = check_cuda(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_planes_post, PP_THREADS, PP_SMEM), "cudaOccupancy");
+        if (rc_ == PSLAM_OK && per_sm < 1) rc_ = set_error(c, PSLAM_E_INVALID, "planes post: kernel does not fit on an SM");
+        if (rc_ != PSLAM_OK) { planepost_free(c); return rc_; }
+        B.workers = sms * per_sm;
+    }
     {   // mt19937(12345) seeded and regenerated once (what the first draw of every RANSAC run sees)
         uint32_t mt[624];
         mt[0] = 12345u;
@@ -600,6 +731,7 @@ static int planepost_alloc(pslam_ctx* c) {
     int rc;
     if ((rc = B.d_coef.reserve(c, nb * B.maxp * 4)) || (rc = B.d_valid.reserve(c, nb * B.maxp)) || (rc = B.d_npts.reserve(c, nb * B.maxp)) ||
         (rc = B.d_stats.reserve(c, nb * B.maxp * 2)) || (rc = B.d_pts.reserve(c, nb * B.maxp * (size_t)PP_SLOTS * 3)) ||
+        (rc = B.d_work.reserve(c, nb * B.maxp)) || (rc = B.d_ctl.reserve(c, 2)) ||
         (rc = B.d_cloud.reserve(c, nb * np * 3)) || (rc = B.d_dist.reserve(c, nb * (np + 2))) ||
         (rc = B.d_ix.reserve(c, nb * ni * 3)) || (rc = B.d_iy.reserve(c, nb * ni * 3)) || (rc = B.d_nrm.reserve(c, nb * np * 3))) {
         planepost_free(c);
@@ -630,13 +762,12 @@ int pslam_planes_post_batch_dev(pslam_ctx* c, const uint16_t* d_depth, int nfram
     PlanePostBuffers& B = *c->planepost;
     cudaStream_t st = c->stream;
     const PPCam K{c->cfg.fx, c->cfg.fy, c->cfg.cx, c->cfg.cy, c->cfg.depth_scale};
-    const size_t smem = (size_t)PP_SLOTS * (3 * 8 + 4 + 4 + 3 * 4 + 4) + 624 * 4;
-    PSLAM_CUDA(c, cudaFuncSetAttribute(k_planes_post, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     PSLAM_CUDA(c, cudaMemsetAsync(d_status, 0, (size_t)nframes * 4, st));
-    PSLAM_LAUNCH(c, "planes_post", k_planes_post<<<dim3(B.maxp, nframes), PP_THREADS, smem, st>>>(d_depth, c->cfg.width, c->cfg.height, K, d_planes, d_nplanes, d_member_idx,
-                 d_member_off, B.maxp, (double)dist_th, B.d_coef, B.d_valid, B.d_npts, B.d_pts, B.d_stats, d_status));
-    PSLAM_LAUNCH(c, "planes_compact", k_planes_compact<<<nframes, 256, 0, st>>>(B.maxp, cap_pts, B.d_coef, B.d_valid, B.d_npts, B.d_pts, d_n_kept, d_src, d_coef, d_pt_off,
-                 d_pts, d_status));
+    PSLAM_LAUNCH(c, "planes_worklist", k_planes_worklist<<<1, 1024, 0, st>>>(nframes, B.maxp, d_nplanes, B.d_work, B.d_ctl));
+    PSLAM_LAUNCH(c, "planes_post", k_planes_post<<<B.workers, PP_THREADS, PP_SMEM, st>>>(d_depth, c->cfg.width, c->cfg.height, K, d_planes, B.d_work, B.d_ctl,
+                 d_member_idx, d_member_off, B.maxp, (double)dist_th, B.d_coef, B.d_valid, B.d_npts, B.d_pts, B.d_stats, d_status));
+    PSLAM_LAUNCH(c, "planes_compact", k_planes_compact<<<nframes, 256, 0, st>>>(B.maxp, cap_pts, d_nplanes, B.d_coef, B.d_valid, B.d_npts, B.d_pts, d_n_kept, d_src,
+                 d_coef, d_pt_off, d_pts, d_status));
     PSLAM_CUDA(c, cudaGetLastError());
     return PSLAM_OK;
 }
