@@ -283,8 +283,11 @@ int pslam_track_sequence(pslam_ctx* ctx, const uint8_t* gray, const uint16_t* de
  *   - the chain does not stop at a failed frame: the following frames are tracked from the kept pose.
  *   - the last frame's map points for SearchByProjection(cur, last) / MatchORBPoints are the frame's matches at the end of the frame with the
  *     local-map outliers flagged (mvbOutlier), as the reference's mLastFrame holds them.
- *   - not modelled: key-frame insertion, MapPlane::UpdateCoefficientsAndPoints / FlagMatchedPlanePoints between frames (:294-303), UpdateLastFrame's
- *     reference-key-frame pose, the mnLastRelocFrameId + 2 window sizes; the snapshot (map, reference key frame, Rotation_cm) is fixed for the sequence.
+ *   - MapPlane::UpdateCoefficientsAndPoints(mCurrentFrame, i) after every frame (:296-304) runs when map plane updates are on (see below); by default the
+ *     map planes' clouds are the uploaded ones for the whole call.  Map::FlagMatchedPlanePoints (:294) is not modelled: it only sets
+ *     MapPoint::mbAssociatedWithPlane, which nothing reads (MapPoint::isAssociatedWithPlane, src/MapPoint.cc:181, has no caller).
+ *   - not modelled: key-frame insertion, UpdateLastFrame's reference-key-frame pose, the mnLastRelocFrameId + 2 window sizes; apart from the map plane
+ *     clouds in update mode, the snapshot (map, reference key frame, Rotation_cm) is fixed for the sequence.
  * The snapshot is uploaded once by pslam_track_set_planar_map into state of its own (what pslam_track_set_map uploaded is left alone).  Stage B runs
  * frame after frame on the context's stream with no host synchronisation and no device-to-host copy between frames: every branch is taken on the device.
  * Outputs: Tcw_out [nframes][16]; Rcm_out [nframes][9] = mLastRcm after each frame (may be NULL); stats [nframes][PSLAM_PLANAR_STATS] (may be NULL). */
@@ -322,6 +325,26 @@ int pslam_track_planar_sequence_dev(pslam_ctx* ctx, const uint8_t* d_gray, const
                                     const float* Tcw0, const float* vel0 /* may be NULL */, const float* Rcm0, float* Tcw_out, float* Rcm_out, int32_t* stats);
 int pslam_track_planar_sequence(pslam_ctx* ctx, const uint8_t* gray, const uint16_t* depth, int nframes, const pslam_planar_track_params* params,
                                 const float* Tcw0, const float* vel0, const float* Rcm0, float* Tcw_out, float* Rcm_out, int32_t* stats);
+/* Map plane updates (off by default; off, every output is what the fixed snapshot gives).  pslam_track_planar_set_map_plane_updates(ctx, 1): every later
+ * sequence call runs MapPlane::UpdateCoefficientsAndPoints(mCurrentFrame, i) for each frame plane i with mvpMapPlanes[i] after every frame - frame 0 and
+ * failed frames included, as the reference's Track() does - with the frame's final pose and final associations, on the device (one launch per frame).
+ *   - frame planes matched to one map plane are merged one after the other in ascending i (each merge = the frame cloud at toSE3Quat(mTcw).inverse() plus
+ *     the plane's current cloud at the identity, pcl::VoxelGrid 0.1 m; pslam_map_plane_update_batch's conventions); the next frame's
+ *     SearchMapByCoefficients reads the new clouds.  The SACSegmentation call after the filter writes locals nobody reads and is not reproduced.
+ *   - a map plane holds at most pslam_map_plane_max_points() points: a call in update mode refuses a snapshot plane above that (PSLAM_E_CAPACITY, before
+ *     any work); a merge above it (or with a point beyond the voxel key range) leaves that plane's cloud as it was, and the call still writes every output
+ *     and returns PSLAM_E_CAPACITY at the end.
+ *   - the clouds persist from call to call; pslam_track_set_planar_map resets them to the upload, and so does switching the mode off.
+ * pslam_track_planar_get_map_plane_updates: the context's mode (1 on, 0 off).
+ * pslam_track_planar_map_planes: the current mvPlanePoints of every snapshot map plane in upload order as CSR, pts_off [n + 1], pts [cap][3] (the upload when
+ * the mode is off); PSLAM_E_CAPACITY when pts_off[n] > cap (pts_off is written).  pslam_track_planar_plane_matches: out [nframes][3][pslam_peac_max_planes()]
+ * = each frame's final {mvpMapPlanes, mvpParallelPlanes, mvpVerticalPlanes} (map plane index or -1) from the last call in update mode, nframes <= its
+ * length (what CreateNewKeyFrame reads, src/Tracking.cc:2248-2272): as in TrackLocalMap (:2018-2030), the parallel / vertical associations PoseOptimization
+ * flagged as outliers are dropped, matched planes keep theirs (mvbPlaneOutlier is not returned). */
+int pslam_track_planar_set_map_plane_updates(pslam_ctx* ctx, int on);
+int pslam_track_planar_get_map_plane_updates(const pslam_ctx* ctx);
+int pslam_track_planar_map_planes(pslam_ctx* ctx, int32_t* pts_off, float* pts, int cap);
+int pslam_track_planar_plane_matches(pslam_ctx* ctx, int32_t* out, int nframes);
 
 /* ---- Key-frame descriptor exchange over NVLink peer memory, fused with the Hamming matcher (SURVEY.md section 8e) -------------------
  * The one exchange step of the multi-GPU layout: every rank (one process per GPU) publishes the ORB block of a key frame - descriptors [n][32], key points

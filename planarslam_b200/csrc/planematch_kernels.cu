@@ -12,14 +12,14 @@
 namespace pslam {
 
 __global__ void __launch_bounds__(256) k_plane_pairs(int n_frame, int n_map, const float* __restrict__ pM /*[n_frame][4]*/, const float* __restrict__ map_coef,
-                                                     const int32_t* __restrict__ pts_off, const float* __restrict__ pts, float* __restrict__ angle,
-                                                     float* __restrict__ mind) {
+                                                     const int32_t* __restrict__ pts_begin, const int32_t* __restrict__ pts_end, const float* __restrict__ pts,
+                                                     float* __restrict__ angle, float* __restrict__ mind) {
     const int pair = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (pair >= n_frame * n_map) return;
     const int i = pair / n_map, j = pair - i * n_map;
     const float a = pM[4 * i], b = pM[4 * i + 1], c = pM[4 * i + 2], d = pM[4 * i + 3];
     float res = 100.f;       // the reference keeps the minimum in a double initialised to 100; every candidate is a float value
-    for (int p = pts_off[j] + lane; p < pts_off[j + 1]; p += 32) res = fminf(res, fabsf(a * pts[3 * p] + b * pts[3 * p + 1] + c * pts[3 * p + 2] + d));
+    for (int p = pts_begin[j] + lane; p < pts_end[j]; p += 32) res = fminf(res, fabsf(a * pts[3 * p] + b * pts[3 * p + 1] + c * pts[3 * p + 2] + d));
 #pragma unroll
     for (int o = 16; o; o >>= 1) res = fminf(res, __shfl_xor_sync(0xffffffffu, res, o));
     if (lane == 0) { angle[pair] = a * map_coef[4 * j] + b * map_coef[4 * j + 1] + c * map_coef[4 * j + 2]; mind[pair] = res; }
@@ -46,10 +46,11 @@ __global__ void k_plane_assign(int n_frame, int n_map, const uint8_t* __restrict
     if (m >= 0) atomicAdd(nmatches, 1);
 }
 
-// pM: the frame planes in world coordinates ([n_frame][4]); ang / mind: [n_frame][n_map] scratch; *nmatches is incremented per matched frame plane
-int plane_match_run_dev(pslam_ctx* c, int n_frame, int n_map, const float* pM, const float* map_coef, const uint8_t* map_bad, const int32_t* pts_off, const float* pts,
-                        float* ang, float* mind, float dTh, float aTh, float verTh, float parTh, int32_t* match, int32_t* ver, int32_t* par, int32_t* nmatches) {
-    PSLAM_LAUNCH(c, "plane_pairs", k_plane_pairs<<<(n_frame * n_map + 7) / 8, 256, 0, c->stream>>>(n_frame, n_map, pM, map_coef, pts_off, pts, ang, mind));
+// pM: the frame planes in world coordinates ([n_frame][4]); map plane j's points are pts[pts_begin[j] .. pts_end[j]) (a CSR offset array passes itself and
+// itself + 1; the minimum does not depend on the order); ang / mind: [n_frame][n_map] scratch; *nmatches is incremented per matched frame plane
+int plane_match_run_dev(pslam_ctx* c, int n_frame, int n_map, const float* pM, const float* map_coef, const uint8_t* map_bad, const int32_t* pts_begin,
+                        const int32_t* pts_end, const float* pts, float* ang, float* mind, float dTh, float aTh, float verTh, float parTh, int32_t* match, int32_t* ver, int32_t* par, int32_t* nmatches) {
+    PSLAM_LAUNCH(c, "plane_pairs", k_plane_pairs<<<(n_frame * n_map + 7) / 8, 256, 0, c->stream>>>(n_frame, n_map, pM, map_coef, pts_begin, pts_end, pts, ang, mind));
     PSLAM_LAUNCH(c, "plane_assign", k_plane_assign<<<(n_frame + 63) / 64, 64, 0, c->stream>>>(n_frame, n_map, map_bad, ang, mind, dTh, aTh, verTh, parTh, match, ver, par,
                  nmatches));
     return PSLAM_OK;
@@ -90,7 +91,7 @@ extern "C" int pslam_plane_match(pslam_ctx* c, const float* Tcw, int n_frame, co
     s.zero(d_cnt, st);
     if ((rc = s.check(c)) != PSLAM_OK) return rc;
     int32_t* out_d = s[d_out];
-    plane_match_run_dev(c, n_frame, n_map, s[d_pM], s[d_mc], s[d_bad], s[d_off], s[d_pts], s[d_ang], s[d_min], dTh, aTh, verTh, parTh, out_d, out_d + n_frame,
+    plane_match_run_dev(c, n_frame, n_map, s[d_pM], s[d_mc], s[d_bad], s[d_off], s[d_off] + 1, s[d_pts], s[d_ang], s[d_min], dTh, aTh, verTh, parTh, out_d, out_d + n_frame,
                         out_d + 2 * n_frame, s[d_cnt]);
     std::vector<int32_t> out((size_t)3 * n_frame + 1);
     s.down(out.data(), d_out, st); s.down(out.data() + 3 * n_frame, d_cnt, st);

@@ -170,8 +170,8 @@ int orb_run_dev(pslam_ctx* c, const uint8_t* d_gray, int nframes, pslam_keypoint
 int line_search_run_dev(pslam_ctx* c, int nf, const float* pt, const float* angle, const int32_t* octave, const uint8_t* desc, const uint8_t* has_obs, const float* scale,
                         int n_levels, int nm, const uint8_t* skip, const int32_t* level, const float* view_cos, const float* proj, const uint8_t* mdesc,
                         const uint8_t* m_has_obs, float th, float nnratio, int32_t* assigned, int32_t* nmatches);   // linesearch_kernels.cu
-int plane_match_run_dev(pslam_ctx* c, int n_frame, int n_map, const float* pM, const float* map_coef, const uint8_t* map_bad, const int32_t* pts_off, const float* pts,
-                        float* ang, float* mind, float dTh, float aTh, float verTh, float parTh, int32_t* match, int32_t* ver, int32_t* par,
+int plane_match_run_dev(pslam_ctx* c, int n_frame, int n_map, const float* pM, const float* map_coef, const uint8_t* map_bad, const int32_t* pts_begin,
+                        const int32_t* pts_end, const float* pts, float* ang, float* mind, float dTh, float aTh, float verTh, float parTh, int32_t* match, int32_t* ver, int32_t* par,
                         int32_t* nmatches);                                                                                   // planematch_kernels.cu
 // pose optimisation (pose_pipeline.cu)
 void pose_free(pslam_ctx* c);

@@ -21,6 +21,7 @@
 #include <cstring>
 #include <vector>
 
+#include "mapplane_body.cuh"
 #include "pose_kernels.cuh"
 #include "search_kernels.cuh"
 
@@ -165,6 +166,11 @@ struct PlanarTrackBuffers {
     const float* R_cm = nullptr; bool ready = false;
     // sequence products and chain state
     DevArray<uint8_t> seq, state;
+    // MapPlane::UpdateCoefficientsAndPoints after every frame (pslam_track_planar_set_map_plane_updates): map plane j's current cloud is
+    // seg_pts[seg_begin[j] .. seg_end[j]) with seg_begin[j] = j * MP_SLOTS.  seg_live: the segments hold the current clouds; otherwise the next call in update
+    // mode seeds them from the upload.  rows [rows_frames][3][maxp]: the associations of every frame of the last call in update mode.
+    bool update_planes = false, seg_live = false; int max_plane_pts = 0; std::vector<int32_t> h_off;
+    DevArray<float> seg_pts; DevArray<int32_t> seg_begin, seg_end, rows; int rows_frames = 0;
 };
 
 struct PlanarCam { float fx, fy, cx, cy, bf, min_x, max_x, min_y, max_y, log_scale_factor; };
@@ -414,13 +420,15 @@ __global__ void __launch_bounds__(256) k_planar_pack(int mode, int32_t* __restri
 // the outlier sweeps.  mode 1 (TranslationWithMotionModel :1795-1855): outlier points / lines lose their match and are skipped by the local-map searches
 // (mnLastFrameSeen); nmatchesMap / line / plane inliers; fail below 3 (pose back to the prediction).  mode 0 (TrackLocalMap :1971-2044): outlier points
 // keep their match with mvbOutlier set (the next frame's last-frame flags); mnMatchesInliers; fail below 7; a tracked frame drops the matches of points
-// without observations ("Clean VO matches", :320-327).  Parallel / vertical outliers are cleared in both (they are not read again).
+// without observations ("Clean VO matches", :320-327).  Mode 0 also drops the parallel / vertical associations PoseOptimization flagged
+// (mvpParallelPlanes / mvpVerticalPlanes[i] = NULL, :2018-2030); matched planes keep theirs (the reference's nulling is commented out).  Mode 1 has no
+// parallel / vertical edges, so its identical loop (:1828-1840) has nothing to drop.
 __global__ void __launch_bounds__(256) k_planar_sweep(int mode, int32_t* __restrict__ st, const PoseHeaderDev* __restrict__ hdr, const PoseOutDev* __restrict__ out,
                                                       const uint8_t* __restrict__ f_pt, const uint8_t* __restrict__ f_line, const uint8_t* __restrict__ f_plane,
                                                       PlanarEdges E, int32_t* __restrict__ matches, uint8_t* __restrict__ outl, uint8_t* __restrict__ skip,
                                                       const uint8_t* __restrict__ has_obs, int32_t* __restrict__ lmatch, uint8_t* __restrict__ lskip,
                                                       const uint8_t* __restrict__ l_has_obs, const int32_t* __restrict__ n_kept, int maxp,
-                                                      const int32_t* __restrict__ match3, float* __restrict__ T, int32_t* __restrict__ stats) {
+                                                      int32_t* __restrict__ match3, float* __restrict__ T, int32_t* __restrict__ stats) {
     __shared__ int s_cnt[3];
     const int tid = threadIdx.x;
     if (!st[0]) {
@@ -456,6 +464,12 @@ __global__ void __launch_bounds__(256) k_planar_sweep(int mode, int32_t* __restr
         }
         s_cnt[1] = c_l; s_cnt[2] = c_p;
     }
+    if (mode == 0)             // after the plane count above read match3; edge e of family f came from frame plane plane_of_edge[f * maxp + e]
+        for (int f = 1; f < 3; ++f) {
+            const int n_f = f == 1 ? H.n_par : H.n_ver;
+            for (int e = tid; e < n_f; e += 256)
+                if (f_plane[f * maxp + e]) match3[f * maxp + E.plane_of_edge[f * maxp + e]] = -1;
+        }
     __syncthreads();
     if (tid != 0) return;
     const int n_map_in = s_cnt[0], total = s_cnt[0] + s_cnt[1] + s_cnt[2];
@@ -481,6 +495,56 @@ __global__ void k_planar_clean(const int32_t* __restrict__ st, int32_t* __restri
     if (!st[1] || i >= min(*n_kp, cap)) return;
     const int m = matches[i];
     if (m >= 0 && !has_obs[m]) { matches[i] = -1; outl[i] = 0; }
+}
+
+// update mode, before the first frame: map plane j's uploaded cloud into its segment
+__global__ void __launch_bounds__(256) k_planar_seed_planes(const int32_t* __restrict__ p_off, const float* __restrict__ p_pts, float* __restrict__ seg_pts,
+                                                            int32_t* __restrict__ seg_begin, int32_t* __restrict__ seg_end) {
+    const int j = blockIdx.x, b = p_off[j], n = p_off[j + 1] - b;
+    for (int k = threadIdx.x; k < 3 * n; k += 256) seg_pts[(size_t)j * MP_SLOTS * 3 + k] = p_pts[(size_t)b * 3 + k];
+    if (threadIdx.x == 0) { seg_begin[j] = j * MP_SLOTS; seg_end[j] = j * MP_SLOTS + n; }
+}
+
+// MapPlane::UpdateCoefficientsAndPoints(mCurrentFrame, i) for every frame plane i with mvpMapPlanes[i] (src/Tracking.cc:296-304), after every frame, tracked
+// or not, at the frame's final pose.  CTA j = map plane j walks the frame planes in ascending i; each i with match3[i] == j rebuilds the cloud from the frame
+// cloud i at T = toSE3Quat(mTcw).inverse() and the current cloud at the identity, one merge after the other as the reference's loop does.  A merge that
+// does not fit (more than MP_SLOTS voxels, or a point beyond the key range) leaves the cloud as it was and sets bit 0 of the frame's status.  CTA 0 also
+// records the frame's associations (row [3][maxp], the match3 layout).  Segments are read and written in place: no restrict on seg_pts.
+__global__ void __launch_bounds__(MP_THREADS, 1) k_planar_map_plane_update(const float* __restrict__ T, const int32_t* __restrict__ match3,
+                                                                          const int32_t* __restrict__ n_kept, int maxp, const int32_t* __restrict__ f_off,
+                                                                          const float* __restrict__ f_pts, int n_planes, float* seg_pts,
+                                                                          const int32_t* __restrict__ seg_begin, int32_t* seg_end, int32_t* __restrict__ row,
+                                                                          int32_t* __restrict__ status) {
+    extern __shared__ __align__(16) unsigned char mp_smem[];
+    __shared__ int s_flag, s_n;
+    __shared__ double s_T[12], s_I[12];
+    const int j = blockIdx.x, tid = threadIdx.x;
+    if (j == 0) for (int k = tid; k < 3 * maxp; k += MP_THREADS) row[k] = match3[k];
+    if (j >= n_planes) return;
+    const int nk = min(*n_kept, maxp);
+    bool any = false;
+    for (int i = 0; i < nk; ++i) any |= match3[i] == j;
+    if (!any) return;
+    if (tid == 0) mp_pose_inverse(T, s_T);
+    if (tid < 12) s_I[tid] = tid % 5 == 0 ? 1.0 : 0.0;          // the identity's rows
+    const MpTable S = mp_table(mp_smem, &s_flag, &s_n);
+    const int b = seg_begin[j];
+    for (int i = 0; i < nk; ++i) {
+        if (match3[i] != j) continue;
+        mp_clear(S, tid);
+        __syncthreads();                                         // also publishes s_T, s_I and the previous merge's cloud and seg_end
+        mp_add(S, tid, f_pts, f_off[i], f_off[i + 1], s_T);
+        mp_add(S, tid, seg_pts, b, seg_end[j], s_I);
+        mp_sort(S, tid);
+        const int N = s_n;
+        if (s_flag || N > MP_SLOTS) {
+            if (tid == 0) atomicOr(status, 1);
+        } else {
+            mp_emit(S, tid, MP_SLOTS, seg_pts + (size_t)b * 3);
+            if (tid == 0) seg_end[j] = b + N;
+        }
+        __syncthreads();
+    }
 }
 
 void track_free(pslam_ctx* c) {
@@ -650,6 +714,10 @@ int pslam_track_set_planar_map(pslam_ctx* c, const pslam_planar_map* pm) {
     if (!c->ptrack) c->ptrack = new PlanarTrackBuffers();
     PlanarTrackBuffers& B = *c->ptrack;
     B.ready = false;
+    B.seg_live = false;                                           // the map planes' clouds restart from this upload
+    B.h_off.assign(p->pts_off, p->pts_off + (p->n ? p->n + 1 : 0));
+    B.max_plane_pts = 0;
+    for (int j = 0; j < p->n; ++j) B.max_plane_pts = std::max(B.max_plane_pts, p->pts_off[j + 1] - p->pts_off[j]);
     const size_t nm = (size_t)m->n, nl = (size_t)l->n, np = (size_t)p->n, npts = np ? (size_t)p->pts_off[p->n] : 0, nr = (size_t)pm->n_ref_lines;
     Slab s;
     const auto pos = s.add<float>(nm * 3), normal = s.add<float>(nm * 3), max_d = s.add<float>(nm), min_d = s.add<float>(nm);
@@ -694,8 +762,10 @@ int pslam_track_planar_sequence_dev(pslam_ctx* c, const uint8_t* d_gray, const u
     if (!d_gray || !d_depth || !prm || !Tcw0 || !Rcm0 || !Tcw_out || nframes < 1 || nframes > c->cfg.max_batch || prm->max_lines < 1 || prm->max_lines > 64)
         return set_error(c, PSLAM_E_INVALID, "bad planar tracking arguments");
     if (!c->ptrack || !c->ptrack->ready) return set_error(c, PSLAM_E_INVALID, "no planar map snapshot (pslam_track_set_planar_map)");
-    PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     PlanarTrackBuffers& B = *c->ptrack;
+    const bool upd = B.update_planes;
+    if (upd && B.max_plane_pts > MP_SLOTS) return set_error(c, PSLAM_E_CAPACITY, "map plane updates: a snapshot plane has more points than pslam_map_plane_max_points()");
+    PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     const pslam_track_params& bp = prm->base;
     const OrbGeom& g = c->geom;
     const int cap = std::min(pslam_orb_max_keypoints(c), SEARCH_MAX_KP), maxp = pslam_peac_max_planes(c), n_sn = pslam_surface_normals_count(c);
@@ -763,9 +833,21 @@ int pslam_track_planar_sequence_dev(pslam_ctx* c, const uint8_t* d_gray, const u
     const auto kp_of_edge = w.add<int32_t>(cap), line_of_edge = w.add<int32_t>(ml), plane_of_edge = w.add<int32_t>(3 * (size_t)maxp);
     const auto T_all = w.add<float>(nf * 16), R_all = w.add<float>(nf * 9);
     const auto stats = w.add<int32_t>(nf * PSLAM_PLANAR_STATS);
+    const auto mpst = w.add<int32_t>(upd ? nf : 0);              // map plane update status per frame
     int rc;
     if ((q.bytes() > B.seq.cap || w.bytes() > B.state.cap)) PSLAM_CUDA(c, cudaStreamSynchronize(st));     // an earlier call may still read the old buffers
     if ((rc = q.alloc(c, B.seq)) || (rc = w.alloc(c, B.state))) return rc;
+    const size_t np = (size_t)B.n_planes;
+    if (upd) {
+        if ((rc = B.rows.reserve(c, nf * 3 * maxp))) return rc;
+        if (!B.seg_live) {
+            if ((rc = B.seg_pts.reserve(c, np * MP_SLOTS * 3)) || (rc = B.seg_begin.reserve(c, np)) || (rc = B.seg_end.reserve(c, np))) return rc;
+            if (np) PSLAM_LAUNCH(c, "planar_seed_planes", k_planar_seed_planes<<<B.n_planes, 256, 0, st>>>(B.p_off, B.p_pts, B.seg_pts, B.seg_begin, B.seg_end));
+            B.seg_live = true;
+        }
+        PSLAM_CUDA(c, cudaFuncSetAttribute(k_planar_map_plane_update, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MP_SMEM));
+        B.rows_frames = 0;
+    }
     // ---- stage A: the Frame constructor's products for every frame of the sequence ----
     PSLAM_LAUNCH(c, "track_fill", k_track_fill<<<(nframes + 255) / 256, 256, 0, st>>>(q[seed], nframes, (int32_t)prm->line_seed));
     if ((rc = pslam_peac_run_batch_dev(c, d_depth, nframes, q[labels], q[planes], q[npl], q[members], q[moff])) != PSLAM_OK) return rc;
@@ -786,6 +868,7 @@ int pslam_track_planar_sequence_dev(pslam_ctx* c, const uint8_t* d_gray, const u
     const int32_t n_sn_i = n_sn;
     w.up(nsn, &n_sn_i, st); w.up(scale, c->scale.data(), st, g.nlevels); w.up(isig, c->inv_sigma2.data(), st, g.nlevels);
     w.zero(scalar, st); w.zero(stats, st); w.zero(outl, st);
+    if (upd) w.zero(mpst, st);
     if ((rc = w.check(c)) != PSLAM_OK) return rc;
     PSLAM_CUDA(c, cudaStreamSynchronize(st));        // the host arguments above may be pageable; nothing is synchronised from here to the end of the sequence
     SearchFrameDev F;
@@ -809,7 +892,8 @@ int pslam_track_planar_sequence_dev(pslam_ctx* c, const uint8_t* d_gray, const u
         PSLAM_LAUNCH(c, "planar_plane_world", k_planar_plane_world<<<(maxp + 127) / 128, 128, 0, st>>>(S, Tp, q[ppcoef] + (size_t)t * maxp * 4, q[ppn] + t, maxp, w[pM],
                      w[found3], w[cnt] + 2));
         if (B.n_planes > 0)
-            plane_match_run_dev(c, maxp, B.n_planes, w[pM], B.p_coef, B.p_bad, B.p_off, B.p_pts, w[pang], w[pmind], prm->plane_dist_ref, prm->plane_ang_ref,
+            plane_match_run_dev(c, maxp, B.n_planes, w[pM], B.p_coef, B.p_bad, upd ? B.seg_begin : B.p_off, upd ? B.seg_end : B.p_off + 1,
+                                upd ? B.seg_pts : B.p_pts, w[pang], w[pmind], prm->plane_dist_ref, prm->plane_ang_ref,
                                 prm->plane_ver_th, prm->plane_par_th, w[found3], w[found3] + 2 * maxp, w[found3] + maxp, w[cnt] + 2);
         PSLAM_LAUNCH(c, "planar_plane_merge", k_planar_plane_merge<<<(3 * maxp + 127) / 128, 128, 0, st>>>(w[found3], w[match3], 3 * maxp));
         return PSLAM_OK;
@@ -884,19 +968,27 @@ int pslam_track_planar_sequence_dev(pslam_ctx* c, const uint8_t* d_gray, const u
         // the velocity of a tracked frame (not after frame 0: frame 1 uses vel0), mLastRcm from the final pose
         PSLAM_LAUNCH(c, "track_pose_algebra", k_track_pose_algebra<<<1, 32, 0, st>>>(Tp, 1, 0, w[T_all] + 16 * (size_t)t, t > 0 ? S + 1 : S + 3));
         PSLAM_LAUNCH(c, "planar_rotation", k_planar_rotation<<<1, 32, 0, st>>>(t > 0 ? 1 : 2, w[mh], B.R_cm, w[Rcm], w[Rcw], Tp, w[R_all] + 9 * (size_t)t));
+        if (upd)       // (:294-304) with the frame's final pose and final mvpMapPlanes
+            PSLAM_LAUNCH(c, "planar_map_plane_update", k_planar_map_plane_update<<<std::max(B.n_planes, 1), MP_THREADS, MP_SMEM, st>>>(Tp, w[match3], q[ppn] + t, maxp,
+                         q[ppoff] + (size_t)t * (maxp + 1), q[pppts] + (size_t)t * cap_pts * 3, B.n_planes, B.seg_pts, B.seg_begin, B.seg_end,
+                         B.rows + (size_t)t * 3 * maxp, w[mpst] + t));
     }
     PSLAM_CUDA(c, cudaGetLastError());
     int32_t sc[2] = {0, 0};
-    std::vector<int32_t> pst(nf);
+    std::vector<int32_t> pst(nf), mps(upd ? nf : 0);
     PSLAM_CUDA(c, cudaMemcpyAsync(Tcw_out, w[T_all], nf * 64, cudaMemcpyDeviceToHost, st));
     if (Rcm_out) PSLAM_CUDA(c, cudaMemcpyAsync(Rcm_out, w[R_all], nf * 36, cudaMemcpyDeviceToHost, st));
     if (stats_out) PSLAM_CUDA(c, cudaMemcpyAsync(stats_out, w[stats], nf * PSLAM_PLANAR_STATS * 4, cudaMemcpyDeviceToHost, st));
     PSLAM_CUDA(c, cudaMemcpyAsync(sc, w[scalar], sizeof sc, cudaMemcpyDeviceToHost, st));
     PSLAM_CUDA(c, cudaMemcpyAsync(pst.data(), q[ppst], nf * 4, cudaMemcpyDeviceToHost, st));
+    if (upd) PSLAM_CUDA(c, cudaMemcpyAsync(mps.data(), w[mpst], nf * 4, cudaMemcpyDeviceToHost, st));
     PSLAM_CUDA(c, cudaStreamSynchronize(st));
+    if (upd) B.rows_frames = nframes;
     if (sc[1]) return set_error(c, PSLAM_E_CAPACITY, "more than 128 candidates in one search window");
     for (int f = 0; f < nframes; ++f)
         if (pst[f] & (32 | 64)) return set_error(c, PSLAM_E_CAPACITY, "planar tracking: more plane voxels than the per-frame capacity");
+    for (int f = 0; f < (int)mps.size(); ++f)
+        if (mps[f]) return set_error(c, PSLAM_E_CAPACITY, "map plane updates: a merged cloud exceeds pslam_map_plane_max_points() voxels (the plane kept its cloud)");
     return PSLAM_OK;
 }
 
@@ -905,6 +997,8 @@ int pslam_track_planar_sequence(pslam_ctx* c, const uint8_t* gray, const uint16_
     if (!c) return PSLAM_E_INVALID;
     if (!gray || !depth || nframes < 1 || nframes > c->cfg.max_batch) return set_error(c, PSLAM_E_INVALID, "bad planar tracking arguments");
     if (!c->ptrack || !c->ptrack->ready) return set_error(c, PSLAM_E_INVALID, "no planar map snapshot (pslam_track_set_planar_map)");
+    if (c->ptrack->update_planes && c->ptrack->max_plane_pts > MP_SLOTS)       // refused before the frames are staged
+        return set_error(c, PSLAM_E_CAPACITY, "map plane updates: a snapshot plane has more points than pslam_map_plane_max_points()");
     PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
     const size_t npx = (size_t)c->cfg.width * c->cfg.height;
     Slab s;
@@ -917,6 +1011,56 @@ int pslam_track_planar_sequence(pslam_ctx* c, const uint8_t* gray, const uint16_
     rc = pslam_track_planar_sequence_dev(c, s[dg], s[dd], nframes, prm, Tcw0, vel0, Rcm0, Tcw_out, Rcm_out, stats_out);
     const int src = s.sync(c, c->stream);
     return rc != PSLAM_OK ? rc : src;
+}
+
+int pslam_track_planar_set_map_plane_updates(pslam_ctx* c, int on) {
+    if (!c) return PSLAM_E_INVALID;
+    if (!c->ptrack) c->ptrack = new PlanarTrackBuffers();
+    PlanarTrackBuffers& B = *c->ptrack;
+    if (!on) B.seg_live = false;                                  // mode off: the uploaded clouds; a later update-mode call starts from them again
+    B.update_planes = on != 0;
+    return PSLAM_OK;
+}
+
+int pslam_track_planar_get_map_plane_updates(const pslam_ctx* c) {
+    if (!c) return PSLAM_E_INVALID;
+    return c->ptrack && c->ptrack->update_planes ? 1 : 0;
+}
+
+int pslam_track_planar_map_planes(pslam_ctx* c, int32_t* pts_off, float* pts, int cap) {
+    if (!c) return PSLAM_E_INVALID;
+    if (!c->ptrack || !c->ptrack->ready || !pts_off || cap < 0 || (cap && !pts)) return set_error(c, PSLAM_E_INVALID, "bad map plane readback (or no planar map snapshot)");
+    PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
+    PlanarTrackBuffers& B = *c->ptrack;
+    const int n = B.n_planes;
+    cudaStream_t st = c->stream;
+    const bool seg = B.update_planes && B.seg_live;
+    std::vector<int32_t> end(n);
+    if (seg && n) {
+        PSLAM_CUDA(c, cudaMemcpyAsync(end.data(), B.seg_end, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+        PSLAM_CUDA(c, cudaStreamSynchronize(st));
+    }
+    pts_off[0] = 0;
+    for (int j = 0; j < n; ++j) pts_off[j + 1] = pts_off[j] + (seg ? end[j] - j * MP_SLOTS : B.h_off[j + 1] - B.h_off[j]);
+    if (pts_off[n] > cap) return set_error(c, PSLAM_E_CAPACITY, "map plane readback: more points than cap (pts_off holds the sizes)");
+    for (int j = 0; j < n; ++j) {
+        const size_t k = (size_t)(pts_off[j + 1] - pts_off[j]);
+        const float* src = seg ? B.seg_pts + (size_t)j * MP_SLOTS * 3 : B.p_pts + (size_t)B.h_off[j] * 3;
+        if (k) PSLAM_CUDA(c, cudaMemcpyAsync(pts + (size_t)pts_off[j] * 3, src, k * 12, cudaMemcpyDeviceToHost, st));
+    }
+    PSLAM_CUDA(c, cudaStreamSynchronize(st));
+    return PSLAM_OK;
+}
+
+int pslam_track_planar_plane_matches(pslam_ctx* c, int32_t* out, int nframes) {
+    if (!c) return PSLAM_E_INVALID;
+    if (!c->ptrack || c->ptrack->rows_frames < 1 || !out || nframes < 1 || nframes > c->ptrack->rows_frames)
+        return set_error(c, PSLAM_E_INVALID, "plane association readback: no call in map plane update mode, or nframes beyond its length");
+    PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
+    const size_t maxp = (size_t)pslam_peac_max_planes(c);
+    PSLAM_CUDA(c, cudaMemcpyAsync(out, c->ptrack->rows, (size_t)nframes * 3 * maxp * 4, cudaMemcpyDeviceToHost, c->stream));
+    PSLAM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSLAM_OK;
 }
 
 }  // extern "C"

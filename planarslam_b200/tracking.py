@@ -93,14 +93,33 @@ class PlanarTracker:
     """PlanarSLAM's Tracking::Track() on the device (include/pslam_abi.h pslam_track_planar_*): Manhattan rotation, translation-only motion model, local map
     with point, line and plane edges.  tracker = PlanarTracker(ctx); tracker.set_map(planar_map_dict) (synth_planar_map.build_planar_map shows the keys);
     poses, Rcm, stats = tracker.track(gray [n,H,W] u8, depth [n,H,W] u16, Tcw0, vel0=None, Rcm0=None) - Rcm0 (mLastRcm before frame 0) defaults to
-    R_cw(Tcw0) * Rotation_cm, the Manhattan frame seen from the start pose."""
+    R_cw(Tcw0) * Rotation_cm, the Manhattan frame seen from the start pose.
+    update_map_planes: MapPlane::UpdateCoefficientsAndPoints after every frame, the clouds carried from call to call.  It is a setting of the context: the
+    property reads it back from there, and the constructor changes it only when given True or False (None keeps it).  map_planes() returns the current
+    clouds, plane_matches() each frame's final plane associations of the last call in that mode."""
 
-    def __init__(self, ctx: Context, params: PlanarTrackParams | None = None):
+    def __init__(self, ctx: Context, params: PlanarTrackParams | None = None, update_map_planes: bool | None = None):
         self.ctx, self.params = ctx, params or default_planar_params(width=ctx.cfg.width, height=ctx.cfg.height)
         L = ctx.L
         L.pslam_track_set_planar_map.argtypes = [C.c_void_p, C.c_void_p]
         L.pslam_track_planar_sequence.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p] + [C.c_void_p] * 6
-        self._keep, self.R_cm = None, None
+        L.pslam_track_planar_set_map_plane_updates.argtypes = [C.c_void_p, C.c_int]
+        L.pslam_track_planar_get_map_plane_updates.argtypes = [C.c_void_p]
+        L.pslam_track_planar_map_planes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+        L.pslam_track_planar_plane_matches.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        self._keep, self.R_cm, self._n_planes, self._n_upload, self._last_n = None, None, 0, 0, 0
+        if update_map_planes is not None:
+            self.update_map_planes = update_map_planes
+
+    @property
+    def update_map_planes(self) -> bool:
+        rc = self.ctx.L.pslam_track_planar_get_map_plane_updates(self.ctx.h)
+        self.ctx.check(min(rc, 0))
+        return rc == 1
+
+    @update_map_planes.setter
+    def update_map_planes(self, on: bool):
+        self.ctx.check(self.ctx.L.pslam_track_planar_set_map_plane_updates(self.ctx.h, 1 if on else 0))
 
     def set_map(self, m: dict):
         f32, f64, u8, i32 = np.float32, np.float64, np.uint8, np.int32
@@ -119,6 +138,7 @@ class PlanarTracker:
         s.R_cm[:] = [float(v) for v in self.R_cm.ravel()]
         self._keep = (pt, ln, pl, ref)
         self.ctx.check(self.ctx.L.pslam_track_set_planar_map(self.ctx.h, C.byref(s)))
+        self._n_planes, self._n_upload = len(pl["bad"]), len(pl["pts"])
 
     def track(self, gray: np.ndarray, depth: np.ndarray, Tcw0: np.ndarray, vel0: np.ndarray | None = None, Rcm0: np.ndarray | None = None):
         g, d = np.ascontiguousarray(gray, np.uint8), np.ascontiguousarray(depth, np.uint16)
@@ -132,4 +152,20 @@ class PlanarTracker:
         self.ctx.check(self.ctx.L.pslam_track_planar_sequence(self.ctx.h, g.ctypes.data, d.ctypes.data, n, C.byref(self.params), T0.ctypes.data,
                                                               None if v0 is None else v0.ctypes.data, R0.ctypes.data, poses.ctypes.data, Rcm.ctypes.data,
                                                               stats.ctypes.data))
+        self._last_n = n
         return poses, Rcm, stats
+
+    def map_planes(self):
+        """The map planes' current MapPlane::mvPlanePoints in upload order: (pts_off int32 [n + 1], pts float32 [pts_off[n]][3])."""
+        off = np.zeros(self._n_planes + 1, np.int32)
+        pts = np.zeros((max(self._n_planes * self.ctx.L.pslam_map_plane_max_points(self.ctx.h), self._n_upload), 3), np.float32)
+        self.ctx.check(self.ctx.L.pslam_track_planar_map_planes(self.ctx.h, off.ctypes.data, pts.ctypes.data, len(pts)))
+        return off, pts[:off[-1]].copy()
+
+    def plane_matches(self, nframes: int | None = None) -> np.ndarray:
+        """Each frame's final plane associations from the last track() with update_map_planes: int32 [nframes][3][maxp] = mvpMapPlanes,
+        mvpParallelPlanes, mvpVerticalPlanes (map plane index or -1)."""
+        n = self._last_n if nframes is None else nframes
+        out = np.zeros((n, 3, self.ctx.L.pslam_peac_max_planes(self.ctx.h)), np.int32)
+        self.ctx.check(self.ctx.L.pslam_track_planar_plane_matches(self.ctx.h, out.ctypes.data, n))
+        return out
