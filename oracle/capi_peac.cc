@@ -90,6 +90,21 @@ int orc_planes_post(void* p, const uint16_t* depth, int w, int h, float fx, floa
     }
     return (int)out.size();
 }
+// The same post-processing on plane records given by the caller instead of a PEAC run: n_planes planes, normal_center [n][6] (PeacPlane::normal, ::center),
+// member_off [n + 1] into members (pixel indices).  Outputs as orc_planes_post.
+int orc_planes_post_records(const uint16_t* depth, int w, int h, float fx, float fy, float cx, float cy, float scale, double dist_th, int n_planes,
+                            const double* normal_center, const int32_t* member_off, const int32_t* members, int32_t* src, float* coef, int32_t* npts, float* pts,
+                            int cap_pts, int32_t* stats) {
+    PeacResult r;
+    r.w = w; r.h = h;
+    r.planes.resize(n_planes);
+    r.membership.resize(n_planes);
+    for (int i = 0; i < n_planes; ++i) {
+        for (int k = 0; k < 3; ++k) { r.planes[i].normal[k] = normal_center[6 * i + k]; r.planes[i].center[k] = normal_center[6 * i + 3 + k]; }
+        r.membership[i].assign(members + member_off[i], members + member_off[i + 1]);
+    }
+    return orc_planes_post(&r, depth, w, h, fx, fy, cx, cy, scale, dist_th, src, coef, npts, pts, cap_pts, stats);
+}
 // vSurfaceNormal: out [n][8] = normal xyz, camera position xyz, frame position xy; returns n
 int orc_surface_normals(const uint16_t* depth, int w, int h, float fx, float fy, float cx, float cy, float scale, float* out8, int cap) {
     std::vector<oracle::SurfaceNormal> v;

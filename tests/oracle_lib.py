@@ -507,6 +507,28 @@ def planes_post(depth: np.ndarray, K=(535.4, 539.2, 320.1, 247.6), scale=np.floa
     return out
 
 
+def planes_post_records(depth: np.ndarray, normal_center: np.ndarray, members: list, K, scale, dist_th: float = 0.05):
+    """planes_post on caller-made plane records instead of a PEAC run: normal_center float64 [n][6] (PEAC normal, centre), members = one array of pixel
+    indices per plane.  Same return layout as planes_post."""
+    L = lib()
+    depth = np.ascontiguousarray(depth, np.uint16)
+    h, w = depth.shape
+    L.orc_planes_post_records.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_float] * 5 + [C.c_double, C.c_int] + [C.c_void_p] * 7 + [C.c_int, C.c_void_p]
+    nc = np.ascontiguousarray(normal_center, np.float64).reshape(-1, 6)
+    off = np.concatenate([[0], np.cumsum([len(m) for m in members])]).astype(np.int32)
+    idx = np.ascontiguousarray(np.concatenate(members) if members else np.zeros(0), np.int32)
+    cap = max(len(nc), 1)
+    src, coef, npts, stats = np.zeros(cap, np.int32), np.zeros((cap, 4), np.float32), np.zeros(cap, np.int32), np.zeros((cap, 2), np.int32)
+    pts = np.zeros((200000, 3), np.float32)
+    n = L.orc_planes_post_records(depth.ctypes.data, w, h, K[0], K[1], K[2], K[3], float(np.float32(scale)), dist_th, len(nc), nc.ctypes.data, off.ctypes.data,
+                                  idx.ctypes.data, src.ctypes.data, coef.ctypes.data, npts.ctypes.data, pts.ctypes.data, len(pts), stats.ctypes.data)
+    out, o = [], 0
+    for i in range(n):
+        out.append(dict(src=int(src[i]), coef=coef[i].copy(), points=pts[o:o + npts[i]].copy(), n_inliers=int(stats[i, 0]), n_iterations=int(stats[i, 1])))
+        o += int(npts[i])
+    return out
+
+
 def surface_normals(depth: np.ndarray, K=(535.4, 539.2, 320.1, 247.6), scale=np.float32(1.0 / 5000.0)):
     """Oracle vSurfaceNormal of Frame::ComputePlanes (IntegralImageNormalEstimation AVERAGE_3D_GRADIENT restated; parity unpinned): float32 [n][8] =
     normal xyz (NaN at the borders / depth edges), camera position xyz, frame position xy."""
