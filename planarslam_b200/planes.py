@@ -16,8 +16,11 @@ from ._lib import Context, PLANE_DTYPE
 
 
 class PlaneDetection:
-    def __init__(self, device: int = 0, max_batch: int = 1):
+    def __init__(self, device: int = 0, max_batch: int = 1, **context_overrides):
+        """context_overrides: Context settings other than the camera, e.g. nlevels - the context also holds the ORB pyramid geometry, and every pyramid
+        level must be at least 68 pixels on a side, so frames smaller than 640 x 480 need fewer than the default 8 levels."""
         self.device, self.max_batch = device, max_batch
+        self._overrides = context_overrides
         self._ctx: Context | None = None
         self._key = None
         self._depth = None
@@ -33,7 +36,7 @@ class PlaneDetection:
                 self._ctx.close()
             K = np.asarray(K, np.float32)
             self._ctx = Context(w, h, max(batch, self.max_batch), self.device, fx=float(K[0, 0]), fy=float(K[1, 1]), cx=float(K[0, 2]),
-                                cy=float(K[1, 2]), depth_scale=float(np.float32(scale)))
+                                cy=float(K[1, 2]), depth_scale=float(np.float32(scale)), **self._overrides)
             self._key = key
         return self._ctx
 

@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 
 import oracle_lib
+from depth_cameras import CASES, frames, ramp_band
 from planarslam_b200 import synth
 
 
@@ -99,15 +100,21 @@ def test_extract_line_segments_keylines():
 
 def test_lsd_oracle_other_image_sizes_vs_cv2():
     """1280 x 960 (BASELINE config 5), 320 x 240, and sizes whose 0.8-scaled dimensions are not integers (641 x 479, 333 x 251): the down-scaling samples with
-    step 1 / 0.8 while the destination size is cvRound(0.8 * size) - cv::resize(..., Size(), 0.8, 0.8, INTER_LINEAR_EXACT)."""
-    cases = [synth.render_frame(seed=2, frame=6, width=1280, height=960)[0], synth.render_frame(seed=3, frame=9, width=320, height=240)[0]]
+    step 1 / 0.8 while the destination size is cvRound(0.8 * size) - cv::resize(..., Size(), 0.8, 0.8, INTER_LINEAR_EXACT).  Also every size of
+    depth_cameras.CASES (644 x 482, 640 x 481 and 120 x 117 scale to 515 x 386, 512 x 385 and 96 x 94), and the ramp-band frames whose one rectangle holds
+    more than 8192 pixels (the NFA's large-n path), in all three refinement modes."""
+    cases = [(synth.render_frame(seed=2, frame=6, width=1280, height=960)[0], 100), (synth.render_frame(seed=3, frame=9, width=320, height=240)[0], 100)]
     base = synth.render_frame(seed=5, frame=15)[0]
-    cases += [np.ascontiguousarray(np.pad(base[:479], ((0, 0), (0, 1)), mode="edge")), np.ascontiguousarray(base[100:351, 200:533])]
-    for g in cases:
-        for refine, flag in ((1, cv2.LSD_REFINE_STD), (2, cv2.LSD_REFINE_ADV)):
+    cases += [(np.ascontiguousarray(np.pad(base[:479], ((0, 0), (0, 1)), mode="edge")), 100), (np.ascontiguousarray(base[100:351, 200:533]), 100)]
+    for w, h in sorted({c[:2] for c in CASES.values()}):
+        cases.append((frames(next(k for k, c in CASES.items() if c[:2] == (w, h)), 1)[0][0], 20 if w * h < 320 * 240 else 100))
+    for w, h in ((640, 480), (1280, 960)):
+        cases += [(ramp_band(w, h, tilt, noise=noise), 1) for tilt in (0.0, 3.0) for noise in (0.0, 8.0)]
+    for g, min_segs in cases:
+        for refine, flag in ((0, cv2.LSD_REFINE_NONE), (1, cv2.LSD_REFINE_STD), (2, cv2.LSD_REFINE_ADV)):
             segs, width, prec, nfa = oracle_lib.lsd_detect(g, refine, cap=65536, rect_enum=3)
             ref = cv2.createLineSegmentDetector(flag).detect(g)
-            assert len(segs) == len(ref[0]) > 100, g.shape
+            assert len(segs) == len(ref[0]) >= min_segs, g.shape
             assert np.array_equal(segs, ref[0].reshape(-1, 4)) and np.array_equal(width, ref[1].ravel()) and np.array_equal(prec, ref[2].ravel()), g.shape
             if refine == 2:
                 assert np.array_equal(nfa, ref[3].ravel()), g.shape

@@ -13,6 +13,7 @@ import pytest
 
 import oracle_lib
 import ref_lib
+from depth_cameras import CASES, frames, scale_of
 from planarslam_b200 import synth
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
@@ -74,6 +75,16 @@ def test_oracle_peac_identical_to_compiled_reference_other_cameras_and_sizes():
     assert same(synth.render_frame(seed=2, frame=6, width=1280, height=960)[1], (1070.8, 1078.4, 640.2, 495.2), s5k) >= 2
     assert same(synth.render_frame(seed=2, frame=6, width=320, height=240)[1], (267.7, 269.6, 160.0, 123.8), s5k) >= 1
     assert same(synth.piecewise_planar_depth(3)[:475, :633].copy(), tum, s5k) >= 5                # size not a multiple of the 10 x 10 block
+    # every camera and size of depth_cameras.CASES (TUM2's DepthMapFactor 5208, TAMU, partial blocks at 644x482, 640x481 and 120x117): a room frame and a
+    # piecewise-planar frame through each camera
+    n = 0
+    for name, (w, h, K, factor, _) in sorted(CASES.items()):
+        sc = np.float32(scale_of(factor))
+        pw = synth.piecewise_planar_depth(3, width=max(w, 200), height=max(h, 200), n_rect=6)[:h, :w]
+        n_case = same(frames(name, 1)[1][0], K, sc) + same(np.rint(pw * (factor / 5000.0)).astype(np.uint16), K, sc)
+        assert n_case >= 1, name
+        n += n_case
+    assert n >= 50
 
 
 @pytest.mark.skipif(ref_lib.peac_lib() is None, reason="oracle/_ref/libpeac_ref.so not built and no /root/reference to build it from")

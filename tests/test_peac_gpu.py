@@ -10,9 +10,9 @@ K = np.array([[535.4, 0, 320.1], [0, 539.2, 247.6], [0, 0, 1]], np.float32)
 SCALE = np.float32(1.0 / 5000.0)
 
 
-def _check_frame(res, depth, blocks=None, coarse=None, Kt=(535.4, 539.2, 320.1, 247.6)):
+def _check_frame(res, depth, blocks=None, coarse=None, Kt=(535.4, 539.2, 320.1, 247.6), scale=SCALE):
     labels, planes, members = res
-    orc = oracle_lib.PeacOracle(depth, Kt, SCALE)
+    orc = oracle_lib.PeacOracle(depth, Kt, scale)
     if blocks is not None:
         st, geo, n, valid = blocks
         assert np.array_equal(n, orc.blk_i[:, 0]) and np.array_equal(valid, orc.blk_i[:, 1])
