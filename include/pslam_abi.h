@@ -702,6 +702,31 @@ typedef struct pslam_frame_outputs {
 int pslam_frame_construct_batch(pslam_ctx* ctx, const uint8_t* gray, const uint16_t* depth, int nframes, float depth_factor, float bf, float plane_dist_th,
                                 int max_lines, uint32_t line_seed, const pslam_frame_outputs* out);
 
+/* The same for frames already in device memory (decoded, rendered or predicted on the GPU).  d_gray / d_depth are device pointers, 4-byte aligned; d_out is
+ * the struct above (a host struct) holding device pointers, with the same shapes and the same optional members.  The stages run in the same order as in
+ * pslam_frame_construct_batch and write the same bytes; the call only enqueues on the context's stream: no host synchronisation, no device-to-host copy.
+ * Exception: a call whose batch needs more scratch than the context holds (PEAC's label and member images, 2.4 MB per 640x480 frame) synchronises the
+ * stream once before growing it.  d_status [nframes] receives, per frame, the OR of the PSLAM_FRAME_CAP_* bits below: 0 exactly where
+ * pslam_frame_construct_batch would not report PSLAM_E_CAPACITY for that frame (the outputs are written either way, truncated where a bit is set).
+ * PSLAM_E_INVALID, before any work, for nframes outside [1, max_batch], a null pointer or a misaligned frame pointer. */
+enum {
+    PSLAM_FRAME_CAP_ORB = 1,        /* ORB candidate / key point capacity */
+    PSLAM_FRAME_CAP_PEAC = 2,       /* PEAC planes / region-growing queue */
+    PSLAM_FRAME_CAP_LINES = 4,      /* line segments of the detector */
+    PSLAM_FRAME_CAP_PLANE_PTS = 8   /* voxels of a plane or of the frame above the plane post-processing capacity (cap_plane_pts) */
+};
+int pslam_frame_construct_batch_dev(pslam_ctx* ctx, const uint8_t* d_gray, const uint16_t* d_depth, int nframes, float depth_factor, float bf,
+                                    float plane_dist_th, int max_lines, uint32_t line_seed, const pslam_frame_outputs* d_out, int32_t* d_status);
+
+/* ---- Colour input -------------------------------------------------------------------------------------
+ * Replaces the conversion of  cv::Mat Tracking::GrabImageRGBD(const cv::Mat& imRGB, const cv::Mat& imD, const double& timestamp)   src/Tracking.cc:157-172
+ *   cvtColor(mImGray, mImGray, CV_RGB2GRAY / CV_BGR2GRAY / CV_RGBA2GRAY / CV_BGRA2GRAY)  as mbRGB (Camera.RGB) and the channel count select.
+ * d_color uint8 [nframes][height][width][channels] (channels 3 or 4, dense), d_gray uint8 [nframes][height][width]; both device pointers, 4-byte aligned.
+ * rgb != 0: the first byte of a pixel is R (Camera.RGB: 1), else B.  Bit-exact to OpenCV 4.13's integer path: Y = (9798 R + 19235 G + 3735 B + 2^14) >> 15,
+ * alpha ignored.  Only enqueues on the context's stream; d_gray is the input pslam_frame_construct_batch_dev and the tracking chains take.
+ * PSLAM_E_INVALID for channels other than 3 / 4, nframes outside [1, max_batch], a null or misaligned pointer. */
+int pslam_gray_from_color_batch_dev(pslam_ctx* ctx, const uint8_t* d_color, int channels, int rgb, int nframes, uint8_t* d_gray);
+
 #ifdef __cplusplus
 }
 #endif

@@ -21,6 +21,8 @@ PLANE_DTYPE = np.dtype([("normal", "<f8", 3), ("center", "<f8", 3), ("mse", "<f8
 assert PLANE_DTYPE.itemsize == 72
 
 PSLAM_OK, E_INVALID, E_NO_DEVICE, E_CUDA, E_CAPACITY, E_NCCL = 0, -1, -2, -3, -4, -5
+# PSLAM_FRAME_CAP_*: the per-frame status bits of pslam_frame_construct_batch_dev
+FRAME_CAP_ORB, FRAME_CAP_PEAC, FRAME_CAP_LINES, FRAME_CAP_PLANE_PTS = 1, 2, 4, 8
 
 
 class Config(C.Structure):
@@ -132,6 +134,8 @@ def lib() -> C.CDLL:
     L.pslam_lines_in_frustum.argtypes = [vp, vp, i32, vp, vp, vp, vp, C.c_float, vp, vp, vp, vp]
     L.pslam_compute_stereo_from_rgbd_batch.argtypes = [vp, vp, vp, vp, i32, vp, i32, C.c_float, C.c_float, vp, vp]
     L.pslam_compute_stereo_from_rgbd_batch_dev.argtypes = [vp, vp, vp, vp, i32, vp, i32, C.c_float, C.c_float, vp, vp]
+    L.pslam_gray_from_color_batch_dev.argtypes = [vp, vp, i32, i32, i32, vp]
+    L.pslam_frame_construct_batch_dev.argtypes = [vp, vp, vp, i32, C.c_float, C.c_float, C.c_float, i32, C.c_uint32, vp, vp]
     L.pslam_bow_transform.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]
     L.pslam_bow_set_vocabulary.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp]
     L.pslam_bow_transform_batch.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp]

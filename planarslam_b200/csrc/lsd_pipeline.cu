@@ -202,6 +202,8 @@ int lsd_status_fetch_async(pslam_ctx* c, int nframes, int32_t* h_pinned) {      
     return PSLAM_OK;
 }
 
+const int32_t* lsd_status_dev(const pslam_ctx* c) { return c->lsd ? c->lsd->d_status.ptr : nullptr; }      // the same flags, in HBM
+
 int lsd_keylines_dev(pslam_ctx* c, int nframes, int max_lines, LsdKeyLine* d_kl, double* d_lf, int32_t* d_n) {
     LsdBuffers& B = *c->lsd;
     PSLAM_LAUNCH(c, "lsd_keylines", k_lsd_keylines<<<nframes, 128, B.g.seg_cap * sizeof(float), c->stream>>>(B.g, max_lines, B.d_segs, B.d_nsegs, d_kl, d_lf, d_n));

@@ -185,6 +185,7 @@ void bowdb_free(pslam_ctx* c);
 void bowvoc_free(pslam_ctx* c);
 void frame_free(pslam_ctx* c);
 int lsd_status_fetch_async(pslam_ctx* c, int nframes, int32_t* h_pinned);
+const int32_t* lsd_status_dev(const pslam_ctx* c);
 // PEAC pipeline (peac_pipeline.cu)
 int peac_build_geometry(pslam_ctx* c);
 int peac_alloc(pslam_ctx* c);
