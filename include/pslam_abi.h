@@ -17,6 +17,7 @@
 #ifndef PSLAM_ABI_H_
 #define PSLAM_ABI_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -67,6 +68,10 @@ const char* pslam_last_error(const pslam_ctx* ctx);
 /* Run on a caller-owned CUDA stream (cudaStream_t / CUstream as void*); NULL restores the context's own. */
 int pslam_set_stream(pslam_ctx* ctx, void* cuda_stream);
 int pslam_synchronize(pslam_ctx* ctx);
+/* Page-locked host memory for the host-pointer calls' inputs and outputs (their copies then run asynchronously to the host).  *ptr = NULL for 0 bytes.
+ * pslam_host_free releases it (NULL is ignored); the memory outlives the context. */
+int pslam_host_alloc(pslam_ctx* ctx, size_t bytes, void** ptr);
+void pslam_host_free(void* ptr);
 /* Number of kernel launches this context has issued since creation (bench.py's gpu_launches claim). */
 int64_t pslam_launch_count(const pslam_ctx* ctx);
 
@@ -701,6 +706,15 @@ typedef struct pslam_frame_outputs {
 } pslam_frame_outputs;
 int pslam_frame_construct_batch(pslam_ctx* ctx, const uint8_t* gray, const uint16_t* depth, int nframes, float depth_factor, float bf, float plane_dist_th,
                                 int max_lines, uint32_t line_seed, const pslam_frame_outputs* out);
+
+/* pslam_frame_construct_batch with two inputs it lacks, same outputs and capacity errors:
+ *   image uint8 [nframes][h][w][channels]: channels 1 is the grey frame; 3 / 4 is the colour frame of Tracking::GrabImageRGBD, uploaded as it is and converted on
+ *     the device as pslam_gray_from_color_batch_dev does (rgb = Camera.RGB).
+ *   line_skip [nframes] (may be NULL): frame f's rand() stream of isLineGood starts at srand(line_seed) advanced by line_skip[f] draws (pslam_lines3d_batch's
+ *     skip).  A caller that replays the reference's single libc stream one frame at a time passes the draws made so far and adds n_rand_drawn afterwards.
+ * channels 1 with line_skip NULL is exactly pslam_frame_construct_batch. */
+int pslam_frame_construct_batch_ex(pslam_ctx* ctx, const uint8_t* image, int channels, int rgb, const uint16_t* depth, int nframes, float depth_factor, float bf,
+                                   float plane_dist_th, int max_lines, uint32_t line_seed, const int32_t* line_skip, const pslam_frame_outputs* out);
 
 /* The same for frames already in device memory (decoded, rendered or predicted on the GPU).  d_gray / d_depth are device pointers, 4-byte aligned; d_out is
  * the struct above (a host struct) holding device pointers, with the same shapes and the same optional members.  The stages run in the same order as in

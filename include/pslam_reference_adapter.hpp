@@ -24,6 +24,8 @@
 //   KeyFrameDatabase::add / erase / clear / DetectLoopCandidates(KeyFrame*, float) / DetectRelocalizationCandidates(Frame*)
 //                                                                                     include/KeyFrameDatabase.h:43-75  src/KeyFrameDatabase.cc:38-305
 //   void ORBextractor::operator()(cv::InputArray, cv::InputArray, vector<cv::KeyPoint>&, cv::OutputArray)   include/ORBextractor.h:59-61
+//   Frame::Frame(imRGB, imGray, imDepth, timeStamp, extractor, voc, K, distCoef, bf, thDepth, depthMapFactor) include/Frame.h:57  src/Frame.cc:55-152
+//                                                                                     (FrameConstructor: fills a default-constructed Frame; batch() for replays)
 //
 // Two reference members read here are protected in the reference (MapPoint::mfMaxDistance / mfMinDistance: the getters return them scaled by 1.2 / 0.8
 // and a float division does not undo a float multiplication): add `friend struct pslam_adapter::ref::Access;` to MapPoint, or two raw getters - see
@@ -32,7 +34,10 @@
 #pragma once
 #include <cmath>
 #include <algorithm>
+#include <chrono>
+#include <cstdio>
 #include <cstring>
+#include <string>
 #include <list>
 #include <map>
 #include <mutex>
@@ -721,6 +726,302 @@ public:
 private:
     int nfeatures; float scaleFactor; int nlevels, iniThFAST, minThFAST;
     pslam_ctx* ctx = nullptr; int w = 0, h = 0;
+};
+
+// Planar_SLAM::Frame's RGB-D constructor  Frame(imRGB, imGray, imDepth, timeStamp, extractor, voc, K, distCoef, bf, thDepth, depthMapFactor)  (include/Frame.h:57,
+// src/Frame.cc:55-152) as a call that fills a default-constructed Frame (Frame::Frame(), src/Frame.cc:19): ExtractORB, ExtractLSD with isLineGood, ComputePlanes,
+// ComputeStereoFromRGBD run in one pslam_frame_construct_batch_ex call; this class writes every member the constructor writes, the Frame statics included
+// (fx ... invfy every frame, mnMinX ... mfGridElement*Inv on the first frame only, as mbInitialComputations says).
+// Refused with std::invalid_argument: a non-zero distCoef[0] (there is no distortion model on this path: the reference would undistort mvKeysUn and the image
+// bounds), a grey image other than CV_8UC1 / CV_8UC3 / CV_8UC4 (colour is converted as Tracking::GrabImageRGBD does, Camera.RGB = rgb), a depth image other than
+// CV_16UC1, or a size other than the constructor's.  A capacity error throws std::runtime_error and leaves the Frame untouched.
+// rand(): the reference's isLineGood draws from the process-wide libc stream, never seeded (srand(1)).  operator() continues one stream from frame to frame
+// (seed, draws()); MapPlane's constructor and Tracking.cc:513 draw from the same stream in the reference, so a caller that runs them reports their draws with
+// advance(n).  batch() starts every frame of the call at the stream position of the call's start and leaves draws() where it was (the replay convention:
+// frame k's start would depend on the draws of frames 0 .. k-1, which are only known after they ran).
+class FrameConstructor {
+public:
+    FrameConstructor(Planar_SLAM::ORBextractor* extractor, int nFeatures, float scaleFactor, int nLevels, int iniThFAST, int minThFAST, const cv::Mat& K,
+                     const cv::Mat& distCoef, float bf, float thDepth, float depthMapFactor, float planeDistanceThreshold, int width, int height, bool rgb = true,
+                     int max_batch = 1, int cap_plane_pts = 16384)
+        : extractor(extractor), K(K.clone()), distCoef(distCoef.clone()), bf(bf), thDepth(thDepth), depthMapFactor(depthMapFactor),
+          planeDistanceThreshold(planeDistanceThreshold), width(width), height(height), rgb(rgb), max_batch(max_batch), cap_plane_pts(cap_plane_pts),
+          nLevels(nLevels), scaleFactor(scaleFactor) {
+        if (K.type() != CV_32F || K.rows != 3 || K.cols != 3) throw std::invalid_argument("FrameConstructor: K must be a 3x3 CV_32F matrix");
+        if (distCoef.empty() || distCoef.type() != CV_32F) throw std::invalid_argument("FrameConstructor: distCoef must be a CV_32F vector");
+        if (distCoef.at<float>(0) != 0.0f) throw std::invalid_argument("FrameConstructor: distorted cameras (distCoef[0] != 0) are not supported");
+        if (max_batch < 1 || cap_plane_pts < 1) throw std::invalid_argument("FrameConstructor: max_batch and cap_plane_pts must be positive");
+        pslam_config cfg;
+        pslam_default_config(&cfg, width, height, max_batch);
+        cfg.nfeatures = nFeatures; cfg.scale_factor = scaleFactor; cfg.nlevels = nLevels; cfg.ini_th_fast = iniThFAST; cfg.min_th_fast = minThFAST;
+        cfg.fx = K.at<float>(0, 0); cfg.fy = K.at<float>(1, 1); cfg.cx = K.at<float>(0, 2); cfg.cy = K.at<float>(1, 2); cfg.depth_scale = depthMapFactor;
+        const int rc = pslam_create(&cfg, &ctx);
+        if (rc != PSLAM_OK) { ctx = nullptr; throw std::runtime_error(rc == PSLAM_E_NO_DEVICE ? "pslam_create failed: no sm_90 GPU" : "pslam_create failed: bad settings"); }
+        capk = pslam_orb_max_keypoints(ctx); maxp = pslam_peac_max_planes(ctx); nsn = pslam_surface_normals_count(ctx);
+        scale.resize(nLevels); inv_scale.resize(nLevels); sigma2.resize(nLevels); inv_sigma2.resize(nLevels);
+        pslam_orb_get_scale_tables(ctx, scale.data(), inv_scale.data(), sigma2.data(), inv_sigma2.data(), nullptr);
+        const size_t nb = (size_t)max_batch, npx = (size_t)width * height;
+        image = stage<uint8_t>(nb * npx * 4); depth = stage<uint16_t>(nb * npx); skip = stage<int32_t>(nb);
+        o.keys = stage<pslam_keypoint>(nb * capk); o.desc = stage<uint8_t>(nb * capk * 32); o.n_keys = stage<int32_t>(nb);
+        o.u_right = stage<float>(nb * capk); o.depth_kp = stage<float>(nb * capk);
+        o.keylines = stage<pslam_keyline>(nb * kMaxLines); o.line_functions = stage<double>(nb * kMaxLines * 3); o.line_desc = stage<uint8_t>(nb * kMaxLines * 32);
+        o.lines3d = stage<pslam_line3d>(nb * kMaxLines); o.n_lines = stage<int32_t>(nb); o.n_rand_drawn = stage<int32_t>(nb);
+        o.n_planes = stage<int32_t>(nb); o.plane_src = stage<int32_t>(nb * maxp); o.plane_coef = stage<float>(nb * maxp * 4);
+        o.plane_pt_off = stage<int32_t>(nb * (maxp + 1)); o.plane_pts = stage<float>(nb * cap_plane_pts * 3); o.cap_plane_pts = cap_plane_pts;
+        o.surface_normals8 = stage<float>(nb * nsn * 8);
+    }
+    ~FrameConstructor() {
+        for (void* p : pinned) pslam_host_free(p);
+        if (ctx) pslam_destroy(ctx);
+    }
+    FrameConstructor(const FrameConstructor&) = delete;
+    FrameConstructor& operator=(const FrameConstructor&) = delete;
+
+    // Frame(imRGB, imGray, imDepth, timeStamp, extractor, voc, K, distCoef, bf, thDepth, depthMapFactor) on F, a default-constructed Frame
+    void operator()(Frame& F, const cv::Mat& imRGB, const cv::Mat& imGray, const cv::Mat& imDepth, const double& timeStamp, Planar_SLAM::ORBVocabulary* voc) {
+        (void)imRGB;                                   // ComputePlanes hands it to PlaneDetection::readColorImage, which nothing reads
+        const int channels = check_image(imGray, imDepth, -1);
+        put(0, imGray, imDepth);
+        skip[0] = (int32_t)mDraws;
+        run(1, channels, timeStamp);
+        const int32_t drawn = o.n_rand_drawn[0];
+        unpack(F, 0, timeStamp, voc);
+        mDraws += drawn;
+    }
+
+    // The constructor for a sequence of frames, max_batch frames per call; frames[i] receives what operator() would put there with the rand() stream at
+    // draws() for every frame (see the class comment).  mnId follows the order of `frames`.
+    void batch(std::vector<Frame*>& frames, const std::vector<cv::Mat>& gray_or_colour, const std::vector<cv::Mat>& depth_images, const std::vector<double>& stamps,
+               Planar_SLAM::ORBVocabulary* voc) {
+        const size_t n = frames.size();
+        if (gray_or_colour.size() != n || depth_images.size() != n || stamps.size() != n) throw std::invalid_argument("FrameConstructor::batch: list lengths differ");
+        const int channels = n ? check_image(gray_or_colour[0], depth_images[0], -1) : 1;
+        for (size_t i = 0; i < n; ++i) {
+            if (!frames[i]) throw std::invalid_argument("FrameConstructor::batch: null Frame");
+            check_image(gray_or_colour[i], depth_images[i], channels);
+        }
+        for (size_t b = 0; b < n; b += (size_t)max_batch) {
+            const int nf = (int)std::min(n - b, (size_t)max_batch);
+            for (int k = 0; k < nf; ++k) { put(k, gray_or_colour[b + k], depth_images[b + k]); skip[k] = (int32_t)mDraws; }
+            run(nf, channels, stamps[b]);
+            for (int k = 0; k < nf; ++k) unpack(*frames[b + k], k, stamps[b + k], voc);
+        }
+    }
+
+    // libc rand() calls made by isLineGood since the stream started (srand(seed)); advance(n) accounts for n draws made elsewhere (a negative n rewinds)
+    int64_t draws() const { return mDraws; }
+    void advance(int64_t n) {
+        if (mDraws + n < 0 || mDraws + n > INT32_MAX) throw std::invalid_argument("FrameConstructor::advance: stream position out of range");
+        mDraws += n;
+    }
+    // host seconds spent in pslam_frame_construct_batch_ex and in filling Frames since construction
+    double call_seconds() const { return mCallSeconds; }
+    double unpack_seconds() const { return mUnpackSeconds; }
+    double support_seconds() const { return mSupportSeconds; }      // the part of unpack_seconds() that rebuilds FrameLine::rndpts3d (compPt3dCov)
+
+    static constexpr int kMaxLines = 40;         // ExtractLineSegment keeps the 40 strongest segments (src/LSDextractor.cpp:18-26)
+    static constexpr uint32_t kSeed = 1;         // libc's stream before any srand
+
+private:
+    template <typename T>
+    T* stage(size_t n) {
+        void* p = nullptr;
+        if (pslam_host_alloc(ctx, std::max(n, (size_t)1) * sizeof(T), &p) != PSLAM_OK) throw std::runtime_error(pslam_last_error(ctx));
+        pinned.push_back(p);
+        return static_cast<T*>(p);
+    }
+    int check_image(const cv::Mat& im, const cv::Mat& dep, int channels) const {
+        const int t = im.type();
+        if (t != CV_8UC1 && t != CV_MAKETYPE(CV_8U, 3) && t != CV_MAKETYPE(CV_8U, 4)) throw std::invalid_argument("FrameConstructor: imGray must be CV_8UC1, CV_8UC3 or CV_8UC4");
+        if (dep.type() != CV_16UC1) throw std::invalid_argument("FrameConstructor: imDepth must be CV_16UC1");
+        if (im.cols != width || im.rows != height || dep.cols != width || dep.rows != height) throw std::invalid_argument("FrameConstructor: image size differs from the constructor's");
+        if (channels > 0 && im.channels() != channels) throw std::invalid_argument("FrameConstructor::batch: grey and colour images mixed in one call");
+        return im.channels();
+    }
+    void put(int k, const cv::Mat& im, const cv::Mat& dep) {
+        const size_t npx = (size_t)width * height, row = (size_t)width * im.channels();
+        for (int y = 0; y < height; ++y) {
+            std::memcpy(image + k * npx * im.channels() + y * row, im.ptr(y), row);
+            std::memcpy(depth + k * npx + (size_t)y * width, dep.ptr(y), (size_t)width * 2);
+        }
+    }
+    void run(int nf, int channels, double first_stamp) {
+        const auto t0 = std::chrono::steady_clock::now();
+        const int rc = pslam_frame_construct_batch_ex(ctx, image, channels, rgb ? 1 : 0, depth, nf, depthMapFactor, bf, planeDistanceThreshold, kMaxLines, kSeed, skip, &o);
+        mCallSeconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+        if (rc == PSLAM_OK) return;
+        char what[96];
+        std::snprintf(what, sizeof what, "FrameConstructor: frame at %.6f%s: ", first_stamp, nf > 1 ? " (or a later one of its batch)" : "");
+        throw std::runtime_error(std::string(what) + pslam_last_error(ctx));
+    }
+
+    // the one unpacking routine of operator() and batch(): slot k of the staged outputs into F, member by member as src/Frame.cc:58-152 writes them
+    void unpack(Frame& F, int k, double timeStamp, Planar_SLAM::ORBVocabulary* voc) {
+        const auto t0 = std::chrono::steady_clock::now();
+        F.mpORBvocabulary = voc; F.mpORBextractorLeft = extractor; F.mpORBextractorRight = static_cast<Planar_SLAM::ORBextractor*>(NULL);
+        F.mTimeStamp = timeStamp; F.mK = K.clone(); F.mDistCoef = distCoef.clone(); F.mbf = bf; F.mThDepth = thDepth;
+        F.mnId = Frame::nNextId++;
+        F.mnScaleLevels = nLevels; F.mfScaleFactor = scaleFactor; F.mfLogScaleFactor = std::log(F.mfScaleFactor);
+        F.mvScaleFactors = scale; F.mvInvScaleFactors = inv_scale; F.mvLevelSigma2 = sigma2; F.mvInvLevelSigma2 = inv_sigma2;
+        set_intrinsics();
+        F.dealWithLine = true;
+
+        // ExtractLSD: ExtractLineSegment, then isLineGood (:189-267)
+        const int NL = o.n_lines[k];
+        const pslam_keyline* kl = o.keylines + (size_t)k * kMaxLines;
+        const pslam_line3d* l3 = o.lines3d + (size_t)k * kMaxLines;
+        F.mvKeylinesUn.resize(NL);
+        F.mvKeyLineFunctions.resize(NL);
+        F.mLdesc = NL ? cv::Mat(NL, 32, CV_8U) : cv::Mat();
+        for (int i = 0; i < NL; ++i) {
+            cv::line_descriptor::KeyLine& L = F.mvKeylinesUn[i];
+            const pslam_keyline& s = kl[i];
+            L.angle = s.angle; L.class_id = s.class_id; L.octave = s.octave; L.pt = cv::Point2f(s.pt_x, s.pt_y); L.response = s.response; L.size = s.size;
+            L.startPointX = s.startPointX; L.startPointY = s.startPointY; L.endPointX = s.endPointX; L.endPointY = s.endPointY;
+            L.sPointInOctaveX = s.sPointInOctaveX; L.sPointInOctaveY = s.sPointInOctaveY; L.ePointInOctaveX = s.ePointInOctaveX; L.ePointInOctaveY = s.ePointInOctaveY;
+            L.lineLength = s.lineLength; L.numOfPixels = s.numOfPixels;
+            const double* lf = o.line_functions + ((size_t)k * kMaxLines + i) * 3;
+            F.mvKeyLineFunctions[i] = Eigen::Vector3d(lf[0], lf[1], lf[2]);
+            std::memcpy(F.mLdesc.ptr(i), o.line_desc + ((size_t)k * kMaxLines + i) * 32, 32);
+        }
+        F.mvDepthLine = std::vector<float>(NL, -1.0f);
+        F.mvLines3D = std::vector<Planar_SLAM::Vector6d>(NL, Eigen::Matrix<double, 6, 1>::Zero());
+        const cv::Mat tmpK = (cv::Mat_<double>(3, 3) << Frame::fx, 0, Frame::cx, 0, Frame::fy, Frame::cy, 0, 0, 1);     // :84-86
+        const uint16_t* raw = depth + (size_t)k * width * height;
+        for (int i = 0; i < NL; ++i) {
+            if (!l3[i].valid) continue;
+            F.mvDepthLine[i] = l3[i].depth;
+            F.mvLines3D[i] << l3[i].A[0], l3[i].A[1], l3[i].A[2], l3[i].B[0], l3[i].B[1], l3[i].B[2];
+            FrameLine tempLine;
+            tempLine.haveDepth = true;
+            const auto ts = std::chrono::steady_clock::now();
+            tempLine.rndpts3d = line_support(F.mvKeylinesUn[i], l3[i], raw, tmpK);
+            mSupportSeconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - ts).count();
+            tempLine.direction = cv::Point3d(l3[i].director[0], l3[i].director[1], l3[i].director[2]);
+            tempLine.direct1 = cv::Point3d(); tempLine.direct2 = cv::Point3d();       // RandomLine3d leaves both unset (src/LineExtractor.cpp:1353-1354)
+            tempLine.p = cv::Point2d(F.mvKeylinesUn[i].endPointX, F.mvKeylinesUn[i].endPointY);
+            tempLine.q = cv::Point2d(F.mvKeylinesUn[i].startPointX, F.mvKeylinesUn[i].startPointY);
+            F.mVF3DLines.push_back(tempLine);
+        }
+
+        // ComputePlanes (:647-753): the kept planes' voxel clouds and refitted coefficients, the surface normals of every other cell of the 3x3 grid
+        const int np = o.n_planes[k];
+        const int32_t* off = o.plane_pt_off + (size_t)k * (maxp + 1);
+        const float* pts = o.plane_pts + (size_t)k * cap_plane_pts * 3;
+        for (int q = 0; q < np; ++q) {
+            Frame::PointCloud cloud;
+            for (int j = off[q]; j < off[q + 1]; ++j) {
+                Frame::PointT p;
+                p.x = pts[3 * j]; p.y = pts[3 * j + 1]; p.z = pts[3 * j + 2];
+                cloud.points.push_back(p);
+            }
+            cloud.width = (unsigned)cloud.points.size(); cloud.height = 1;     // VoxelGrid's output: one row
+            F.mvPlanePoints.push_back(cloud);
+            const float* c = o.plane_coef + ((size_t)k * maxp + q) * 4;
+            F.mvPlaneCoefficients.push_back((cv::Mat_<float>(4, 1) << c[0], c[1], c[2], c[3]));
+        }
+        const float* sn = o.surface_normals8 + (size_t)k * nsn * 8;
+        F.vSurfaceNormal.resize(nsn);
+        for (int i = 0; i < nsn; ++i) {
+            SurfaceNormal& s = F.vSurfaceNormal[i];
+            const float* r = sn + 8 * (size_t)i;
+            s.normal = cv::Point3f(r[0], r[1], r[2]); s.cameraPosition = cv::Point3f(r[3], r[4], r[5]); s.FramePosition = cv::Point2i((int)r[6], (int)r[7]);
+        }
+
+        // ExtractORB, then :99-152
+        const int N = o.n_keys[k];
+        F.N = N;
+        F.NL = NL;
+        F.mvKeys.resize(N);
+        const pslam_keypoint* kp = o.keys + (size_t)k * capk;
+        for (int i = 0; i < N; ++i) {
+            cv::KeyPoint& q = F.mvKeys[i];
+            q.pt.x = kp[i].x; q.pt.y = kp[i].y; q.size = kp[i].size; q.angle = kp[i].angle; q.response = kp[i].response; q.octave = kp[i].octave;
+            q.class_id = kp[i].class_id;
+        }
+        if (N == 0) {                                 // :106-107 (ORBextractor releases the descriptors when it finds nothing)
+            F.mDescriptors.release();
+            mUnpackSeconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+            return;
+        }
+        F.mDescriptors = cv::Mat(N, 32, CV_8U);
+        std::memcpy(F.mDescriptors.ptr(0), o.desc + (size_t)k * capk * 32, (size_t)N * 32);
+        F.mvKeysUn = F.mvKeys;                        // UndistortKeyPoints with distCoef[0] == 0 (:546-548)
+        F.mvuRight.assign(o.u_right + (size_t)k * capk, o.u_right + (size_t)k * capk + N);
+        F.mvDepth.assign(o.depth_kp + (size_t)k * capk, o.depth_kp + (size_t)k * capk + N);
+        F.mvpMapPoints = std::vector<MapPoint*>(N, static_cast<MapPoint*>(NULL));
+        F.mvpMapLines = std::vector<MapLine*>(NL, static_cast<MapLine*>(NULL));
+        F.mvbOutlier = std::vector<bool>(N, false);
+        F.mvbLineOutlier = std::vector<bool>(NL, false);
+        if (Frame::mbInitialComputations) {           // ComputeImageBounds without distortion (:595-600), then :122-132
+            Frame::mnMinX = 0.0f; Frame::mnMaxX = width; Frame::mnMinY = 0.0f; Frame::mnMaxY = height;
+            Frame::mfGridElementWidthInv = static_cast<float>(FRAME_GRID_COLS) / static_cast<float>(Frame::mnMaxX - Frame::mnMinX);
+            Frame::mfGridElementHeightInv = static_cast<float>(FRAME_GRID_ROWS) / static_cast<float>(Frame::mnMaxY - Frame::mnMinY);
+            set_intrinsics();
+            Frame::mbInitialComputations = false;
+        }
+        F.mb = F.mbf / Frame::fx;
+        for (int i = 0; i < N; ++i) {                 // AssignFeaturesToGrid (:155-168)
+            int gx, gy;
+            if (F.PosInGrid(F.mvKeysUn[i], gx, gy)) F.mGrid[gx][gy].push_back(i);
+        }
+        F.mnPlaneNum = (int)F.mvPlanePoints.size();
+        F.mvpMapPlanes = std::vector<MapPlane*>(F.mnPlaneNum, static_cast<MapPlane*>(nullptr));
+        F.mvpParallelPlanes = std::vector<MapPlane*>(F.mnPlaneNum, static_cast<MapPlane*>(nullptr));
+        F.mvpVerticalPlanes = std::vector<MapPlane*>(F.mnPlaneNum, static_cast<MapPlane*>(nullptr));
+        F.mvPlanePointMatches = std::vector<std::vector<MapPoint*>>(F.mnPlaneNum);
+        F.mvPlaneLineMatches = std::vector<std::vector<MapLine*>>(F.mnPlaneNum);
+        F.mvbPlaneOutlier = std::vector<bool>(F.mnPlaneNum, false);
+        F.mvbVerPlaneOutlier = std::vector<bool>(F.mnPlaneNum, false);
+        F.mvbParPlaneOutlier = std::vector<bool>(F.mnPlaneNum, false);
+        mUnpackSeconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    }
+
+    void set_intrinsics() const {                     // :73-78 (and :125-130)
+        Frame::fx = K.at<float>(0, 0); Frame::fy = K.at<float>(1, 1); Frame::cx = K.at<float>(0, 2); Frame::cy = K.at<float>(1, 2);
+        Frame::invfx = 1.0f / Frame::fx; Frame::invfy = 1.0f / Frame::fy;
+    }
+
+    // FrameLine::rndpts3d of an accepted line: the samples of isLineGood (:193-232, the same expressions on the same types) that the fit kept (l.inliers, in
+    // sampling order like RandomLine3d::pts), each with the reference's own compPt3dCov
+    std::vector<RandomPoint3d> line_support(const cv::line_descriptor::KeyLine& kl, const pslam_line3d& l, const uint16_t* raw, const cv::Mat& tmpK) const {
+        const double len = cv::norm(kl.getStartPoint() - kl.getEndPoint());
+        const double numSmp = (double)std::min((int)len, 50);
+        std::vector<cv::Point3d> pts3d;
+        for (int j = 0; j <= numSmp; ++j) {
+            const cv::Point2d pt = kl.getStartPoint() * (1 - j / numSmp) + kl.getEndPoint() * (j / numSmp);
+            if (pt.x < 0 || pt.y < 0 || pt.x >= width || pt.y >= height) continue;
+            int row, col;
+            if ((std::floor(pt.x) == pt.x) && (std::floor(pt.y) == pt.y)) { col = std::max(int(pt.x - 1), 0); row = std::max(int(pt.y - 1), 0); }
+            else { col = int(pt.x); row = int(pt.y); }
+            const float d = (float)raw[(size_t)row * width + col] * depthMapFactor;     // imDepth.convertTo(depth, CV_32F, depthMapFactor) (:81-82)
+            if (d <= 0.01) continue;
+            cv::Point3d p;
+            p.z = d;
+            p.x = (col - Frame::cx) * p.z * Frame::invfx;
+            p.y = (row - Frame::cy) * p.z * Frame::invfy;
+            pts3d.push_back(p);
+        }
+        if ((int)pts3d.size() != l.n_points) throw std::logic_error("FrameConstructor: isLineGood samples differ from the device's");
+        std::vector<RandomPoint3d> r;
+        for (int j = 0; j < (int)pts3d.size() && j < 64; ++j)
+            if (l.inliers >> j & 1) r.push_back(compPt3dCov(pts3d[j], tmpK, 1));
+        if ((int)r.size() != l.n_inliers) throw std::logic_error("FrameConstructor: isLineGood support differs from the device's");
+        return r;
+    }
+
+    Planar_SLAM::ORBextractor* extractor;
+    cv::Mat K, distCoef;
+    float bf, thDepth, depthMapFactor, planeDistanceThreshold;
+    int width, height; bool rgb; int max_batch, cap_plane_pts, nLevels; float scaleFactor;
+    pslam_ctx* ctx = nullptr;
+    int capk = 0, maxp = 0, nsn = 0;
+    std::vector<float> scale, inv_scale, sigma2, inv_sigma2;
+    std::vector<void*> pinned;
+    uint8_t* image = nullptr; uint16_t* depth = nullptr; int32_t* skip = nullptr;
+    pslam_frame_outputs o{};
+    int64_t mDraws = 0;
+    double mCallSeconds = 0, mUnpackSeconds = 0, mSupportSeconds = 0;
 };
 
 }  // namespace ref

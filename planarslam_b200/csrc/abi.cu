@@ -104,6 +104,18 @@ int pslam_synchronize(pslam_ctx* c) {
 
 int64_t pslam_launch_count(const pslam_ctx* c) { return c ? c->launches : 0; }
 
+int pslam_host_alloc(pslam_ctx* c, size_t bytes, void** ptr) {
+    if (!c) return PSLAM_E_INVALID;
+    if (!ptr) return set_error(c, PSLAM_E_INVALID, "host alloc: null pointer");
+    *ptr = nullptr;
+    if (!bytes) return PSLAM_OK;
+    PSLAM_CUDA(c, cudaSetDevice(c->cfg.device));
+    PSLAM_CUDA(c, cudaHostAlloc(ptr, bytes, cudaHostAllocPortable));
+    return PSLAM_OK;
+}
+
+void pslam_host_free(void* ptr) { if (ptr) cudaFreeHost(ptr); }
+
 int pslam_profile_enable(pslam_ctx* c, int on) {
     if (!c) return PSLAM_E_INVALID;
     for (auto& r : c->prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }

@@ -36,6 +36,7 @@ void frame_free(pslam_ctx* c) {
 // Device buffers of one call that are not outputs: PEAC's label image, planes and member lists, the plane post-processing flags, the rand() seeds
 struct FrameScratch {
     int32_t* labels; pslam_plane* planes; int32_t* npl; int32_t* members; int32_t* moff; int32_t* ppst; uint32_t* seed;
+    const int32_t* skip;      // rand() draws to skip per frame after srand(seed), or NULL (every frame starts at its seed)
 };
 
 constexpr int kPlanePtsOverflow = 32 | 64;      // plane post-processing flags that mean "more voxels than the capacity"
@@ -66,7 +67,7 @@ static int extract_lines(pslam_ctx* c, const uint8_t* gray, const uint16_t* dept
     const float cam[4] = {c->cfg.fx, c->cfg.fy, c->cfg.cx, c->cfg.cy};
     int rc;
     if ((rc = pslam_lines_extract_describe_batch_dev(c, gray, nframes, max_lines, o.keylines, o.line_functions, o.line_desc, o.n_lines)) != PSLAM_OK) return rc;
-    return pslam_lines3d_batch_dev(c, o.keylines, o.n_lines, max_lines, depth, nframes, depth_factor, cam, s.seed, nullptr, o.lines3d, o.n_rand_drawn);
+    return pslam_lines3d_batch_dev(c, o.keylines, o.n_lines, max_lines, depth, nframes, depth_factor, cam, s.seed, s.skip, o.lines3d, o.n_rand_drawn);
 }
 
 __global__ void k_frame_seeds(uint32_t* seed, int nframes, uint32_t v) {
@@ -86,12 +87,15 @@ __global__ void k_frame_status(int32_t* status, int nframes, const int32_t* orb,
 
 using namespace pslam;
 
-extern "C" {
+namespace {
 
-int pslam_frame_construct_batch(pslam_ctx* c, const uint8_t* gray, const uint16_t* depth, int nframes, float depth_factor, float bf, float plane_dist_th,
-                                int max_lines, uint32_t line_seed, const pslam_frame_outputs* out) {
+// pslam_frame_construct_batch and pslam_frame_construct_batch_ex: image is grey (channels 1) or colour (3 / 4, converted on the device after its upload),
+// line_skip is NULL or the per-frame rand() draws to skip.  With channels 1 and no skip the launches and copies are those of pslam_frame_construct_batch.
+int construct_host(pslam_ctx* c, const uint8_t* image, int channels, int rgb, const uint16_t* depth, int nframes, float depth_factor, float bf,
+                   float plane_dist_th, int max_lines, uint32_t line_seed, const int32_t* line_skip, const pslam_frame_outputs* out) {
     if (!c) return PSLAM_E_INVALID;
-    if (!gray || !depth || !out || nframes < 1 || nframes > c->cfg.max_batch || max_lines < 1) return set_error(c, PSLAM_E_INVALID, "frame construct: bad arguments");
+    if (!image || !depth || !out || nframes < 1 || nframes > c->cfg.max_batch || max_lines < 1) return set_error(c, PSLAM_E_INVALID, "frame construct: bad arguments");
+    if (channels != 1 && channels != 3 && channels != 4) return set_error(c, PSLAM_E_INVALID, "frame construct: channels must be 1, 3 or 4");
     const int cap = pslam_orb_max_keypoints(c), maxp = pslam_peac_max_planes(c), n_sn = pslam_surface_normals_count(c);
     if (!out->keys || !out->desc || !out->n_keys || !out->u_right || !out->depth_kp || !out->keylines || !out->line_functions || !out->line_desc || !out->lines3d ||
         !out->n_lines || !out->n_planes || !out->plane_src || !out->plane_coef || !out->plane_pt_off || !out->plane_pts || out->cap_plane_pts < 1)
@@ -121,6 +125,8 @@ int pslam_frame_construct_batch(pslam_ctx* c, const uint8_t* gray, const uint16_
     const auto pppts = s.add<float>(nf * cp * 3);
     const auto ppst = s.add<int32_t>(nf);
     const auto sn8 = s.add<float>(out->surface_normals8 ? nf * n_sn * 8 : 0);
+    const auto color_d = s.add<uint8_t>(channels != 1 ? nf * npx * channels : 0);     // empty for grey input and no skips: the slab is unchanged
+    const auto skip_d = s.add<int32_t>(line_skip ? nf : 0);
     int rc;
     if (s.bytes() > B.slab.cap) PSLAM_CUDA(c, cudaStreamSynchronize(c->stream));      // an earlier call's kernels may still read the old slab
     if ((rc = s.alloc(c, B.slab)) || (rc = B.h_status.reserve(c, nf * 4))) return rc;
@@ -135,8 +141,10 @@ int pslam_frame_construct_batch(pslam_ctx* c, const uint8_t* gray, const uint16_
     PSLAM_CUDA(c, cudaEventRecord(B.ev_idle, st));
     PSLAM_CUDA(c, cudaStreamWaitEvent(cs, B.ev_idle, 0));
     s.up(depth_d, depth, st);
-    s.up(gray_d, gray, cs);
+    if (channels == 1) s.up(gray_d, image, cs);
+    else s.up(color_d, image, cs);
     PSLAM_CUDA(c, cudaEventRecord(B.ev_gray, cs));
+    if (line_skip) s.up(skip_d, line_skip, st);
     {   // one rand() stream per frame, all started from the caller's seed (pslam_lines3d_batch documents the single-stream alternative)
         for (int f = 0; f < nframes; ++f) B.h_status[f] = (int32_t)line_seed;
         s.up(seed, reinterpret_cast<const uint32_t*>(B.h_status.ptr), st);
@@ -144,7 +152,7 @@ int pslam_frame_construct_batch(pslam_ctx* c, const uint8_t* gray, const uint16_
     if ((rc = s.check(c)) != PSLAM_OK) return rc;
     pslam_frame_outputs dv = {s[kps], s[desc], s[nk], s[ur], s[dz], s[kl], s[lf], s[ldesc], s[l3d], s[nkl], s[drawn],
                               s[ppn], s[ppsrc], s[ppcoef], s[ppoff], s[pppts], out->cap_plane_pts, out->surface_normals8 ? s[sn8] : nullptr};
-    const FrameScratch sc{s[labels], s[planes], s[npl], s[members], s[moff], s[ppst], s[seed]};
+    const FrameScratch sc{s[labels], s[planes], s[npl], s[members], s[moff], s[ppst], s[seed], line_skip ? s[skip_d] : nullptr};
     // ComputePlanes on the depth frames while the gray frames arrive
     if ((rc = compute_planes(c, s[depth_d], nframes, plane_dist_th, dv, sc)) != PSLAM_OK) return rc;
     PSLAM_CUDA(c, cudaMemcpyAsync(B.h_status + 2 * (size_t)nframes, c->d_status, nf * 4, cudaMemcpyDeviceToHost, st));      // PEAC capacity flags (ORB reuses the array below)
@@ -155,6 +163,7 @@ int pslam_frame_construct_batch(pslam_ctx* c, const uint8_t* gray, const uint16_
     if (out->surface_normals8) s.down(out->surface_normals8, sn8, cs);
     s.down(B.h_status + nframes, ppst, cs);        // plane post-processing capacity flags
     PSLAM_CUDA(c, cudaStreamWaitEvent(st, B.ev_gray, 0));
+    if (channels != 1 && (rc = pslam_gray_from_color_batch_dev(c, s[color_d], channels, rgb, nframes, s[gray_d])) != PSLAM_OK) return rc;   // GrabImageRGBD's cvtColor
     if ((rc = extract_orb(c, s[gray_d], s[depth_d], nframes, depth_factor, bf, dv)) != PSLAM_OK) return rc;
     PSLAM_CUDA(c, cudaMemcpyAsync(B.h_status, c->d_status, nf * 4, cudaMemcpyDeviceToHost, st));                            // ORB capacity flags
     s.down(out->keys, kps, st); s.down(out->desc, desc, st); s.down(out->n_keys, nk, st); s.down(out->u_right, ur, st); s.down(out->depth_kp, dz, st);
@@ -171,6 +180,20 @@ int pslam_frame_construct_batch(pslam_ctx* c, const uint8_t* gray, const uint16_
         if (B.h_status[3 * (size_t)nframes + f]) return set_error(c, PSLAM_E_CAPACITY, "frame construct: more line segments than the internal capacity");
     }
     return PSLAM_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int pslam_frame_construct_batch(pslam_ctx* c, const uint8_t* gray, const uint16_t* depth, int nframes, float depth_factor, float bf, float plane_dist_th,
+                                int max_lines, uint32_t line_seed, const pslam_frame_outputs* out) {
+    return construct_host(c, gray, 1, 0, depth, nframes, depth_factor, bf, plane_dist_th, max_lines, line_seed, nullptr, out);
+}
+
+int pslam_frame_construct_batch_ex(pslam_ctx* c, const uint8_t* image, int channels, int rgb, const uint16_t* depth, int nframes, float depth_factor, float bf,
+                                   float plane_dist_th, int max_lines, uint32_t line_seed, const int32_t* line_skip, const pslam_frame_outputs* out) {
+    return construct_host(c, image, channels, rgb, depth, nframes, depth_factor, bf, plane_dist_th, max_lines, line_seed, line_skip, out);
 }
 
 int pslam_frame_construct_batch_dev(pslam_ctx* c, const uint8_t* d_gray, const uint16_t* d_depth, int nframes, float depth_factor, float bf, float plane_dist_th,
@@ -196,7 +219,7 @@ int pslam_frame_construct_batch_dev(pslam_ctx* c, const uint8_t* d_gray, const u
     if ((rc = s.alloc(c, B.dev_slab)) != PSLAM_OK) return rc;
     pslam_frame_outputs o = *d_out;
     if (!o.n_rand_drawn) o.n_rand_drawn = s[drawn];
-    const FrameScratch sc{s[labels], s[planes], s[npl], s[members], s[moff], s[ppst], s[seed]};
+    const FrameScratch sc{s[labels], s[planes], s[npl], s[members], s[moff], s[ppst], s[seed], nullptr};
     cudaStream_t st = c->stream;
     const unsigned fb = (unsigned)((nframes + 127) / 128);
     PSLAM_LAUNCH(c, "frame_seeds", k_frame_seeds<<<fb, 128, 0, st>>>(sc.seed, nframes, line_seed));
